@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- particle-RK4-steps/s of the hot path on N B200s (contract: see the task statement).
+"""bench.py -- particle-RK4-steps/s of the hot path on N H100s.
 
 One bench "step" = one pass of the hot path over one batch: ``Kernel.execute`` of the workload's kernel list over the
 whole particle set for one output interval (e.g. 144 dt-steps of 600 s = one day), i.e. dt_steps x N_particles
@@ -14,14 +14,18 @@ particle-RK4-steps.
                 compared bit for bit, positions in float32 ulp (N = 1, rank 0)
   cpu_baseline  the time the oracle took for that sample (NumPy restatement of the reference path, one core)
 
-Default (the driver's ``--gpus 1``): the north-star workload ``ns`` (BASELINE.json: 1e7 particles, 1/12 deg 3-D rectilinear
+Default (``--gpus 1``): the north-star workload ``ns`` (BASELINE.json: 1e7 particles, 1/12 deg 3-D rectilinear
 field) as value / e2e / roofline, and BASELINE configs[1..3] (``c2``, ``c3``, ``c4``) as compact blocks under ``extra``.
 ``--gpus N`` > 1 (torchrun): mode R (field replicated, particles sharded, no data-path collective) as value, plus a
 ``mode_d`` block: BASELINE configs[4] (``c5``: the 1/12 deg field cut into N X-slabs, NCCL all-to-all particle migration)
 with a bit-exactness check of the decomposed run against a single GPU.
 
 ``--impl reference`` times the reference arm: the reference's own algorithm (oracle port; the reference is pure Python and
-cannot travel to the GPU box) on all host cores, same ``config``.
+is not installed on GPU machines) on all host cores, same ``config``.
+
+``--dump-outputs DIR`` writes, after the timed steps of every workload of the run, the particle set its device-resident arm
+computed in its last step (rank 0) as ``DIR/<workload>_<column>.npy``: a fixed seeded sample of at most DUMP_ROWS rows of every
+column, so that two builds can be compared output for output on identical inputs.
 """
 
 from __future__ import annotations
@@ -225,7 +229,7 @@ def c5_slab(rank, world, halo, nx=4320, ny=2160, nz=50, nt=2):
 
 # name -> spec.  bytes: algorithmic bytes per particle-step (SURVEY.md 8d / BASELINE.md 4)
 NOTE_AGRID = ("no-reuse byte model: the per-lane corner cache serves most samples on chip, real DRAM traffic is `traffic`; the kernel "
-              "is fp64-issue- and refill-latency-bound, not HBM-bound (profiles/README.md)")
+              "is fp64-issue- and refill-latency-bound, not HBM-bound (DESIGN.md, Roofline)")
 WORKLOADS = {
     "ns": dict(field=ns_field, fkw=dict(nx=4320, ny=2160, nz=50, nt=3), particles=c2_particles, n=10_000_000, dt=600.0,
                nsteps=144, kernels=["AdvectionRK4_3D"], bytes=832, device_field=True, ulp=8, roofline_note=NOTE_AGRID,
@@ -247,7 +251,7 @@ WORKLOADS = {
     "c3": dict(field=c3_field, fkw=dict(nx=1442, ny=1021, nt=3), particles=c3_particles, n=10_000_000, dt=3600.0,
                nsteps=48, kernels=["AdvectionRK4"], bytes=320, ulp=8, ulp_quantile=0.999,
                roofline_note="not HBM-bound: 9 double-precision sin/cos + 5 sqrt + ~8 divisions per sample are the reference's own "
-                             "arithmetic (profiles/README.md: DRAM < 1 % of peak, cos+sin a quarter of the executed instructions)",
+                             "arithmetic (DESIGN.md, Roofline)",
                desc="BASELINE.json configs[2] -- AdvectionRK4, 1e7 particles, curvilinear C-grid ORCA025 shape 1442x1021 T=3, "
                     "f32 lon/lat, CGrid_Velocity + hint/spatial-hash search, spherical"),
     "c3_3d": dict(field=c3_field, fkw=dict(nx=1442, ny=1021, nt=2, nz=31), particles=c3_particles, n=10_000_000, dt=3600.0,
@@ -285,7 +289,7 @@ def config_block(name, w, n_per_gpu):
 
 
 class ClockSampler:
-    """nvidia-smi SM clock + throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi SM clock + throttle reasons during the timed region, and the card's name and power limit."""
 
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")  # fmt: skip
@@ -306,6 +310,12 @@ class ClockSampler:
             self._stop.wait(0.05)
 
     def __enter__(self):
+        try:
+            out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", str(self.index)],
+                                 capture_output=True, text=True, timeout=5).stdout.strip()  # fmt: skip
+            self.device = [s.strip() for s in out.split(",")] if out else None
+        except Exception:
+            self.device = None
         self._t.start()
         return self
 
@@ -314,13 +324,14 @@ class ClockSampler:
         self._t.join(timeout=6)
 
     def summary(self):
+        dev = {"gpu": self.device[0], "power_limit": self.device[-1]} if self.device else {"gpu": None, "power_limit": None}
         if not self.samples:
-            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["unavailable"]}
+            return {**dev, "sm_mhz": None, "sm_max_mhz": None, "reasons": ["unavailable"]}
         sm = [float(s[0]) for s in self.samples if s[0].replace(".", "").isdigit()]
         mx = [float(s[1]) for s in self.samples if s[1].replace(".", "").isdigit()]
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         reasons = [n for i, n in enumerate(names) if any(s[2 + i].lower().startswith("active") for s in self.samples)]
-        return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None, "reasons": reasons,
+        return {**dev, "sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None, "reasons": reasons,
                 "samples": len(self.samples)}  # fmt: skip
 
 
@@ -329,11 +340,11 @@ def measured_peak():
         m = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         return float(m["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet HBM3 bandwidth (not a measured peak)"
 
 
 def dram_traffic_per_launch(workload):
-    """dram__bytes_read+write per launch from the committed ncu capture (profiles/roofline_traffic.json), or None."""
+    """dram__bytes_read+write per launch from an ncu capture stored as profiles/roofline_traffic.json, or None without one."""
     try:
         j = json.load(open(os.path.join(ROOT, "profiles", "roofline_traffic.json")))
         return j.get(workload)
@@ -342,7 +353,7 @@ def dram_traffic_per_launch(workload):
 
 
 def ncu_limiter(workload):
-    """Issue-slot / FP64-pipe utilisation of the workload's kernel from the committed ncu capture (same file), or None: the
+    """Issue-slot / FP64-pipe utilisation of the workload's kernel from that ncu capture (same file), or None: the
     byte model of `roofline` assumes no reuse, these say what the kernel is actually bound by."""
     try:
         j = json.load(open(os.path.join(ROOT, "profiles", "roofline_traffic.json")))
@@ -518,7 +529,25 @@ def build_field(name, w, *, device=None, host=False, threads=None):
     return w["field"](**w["fkw"])
 
 
-def run_gpu_workload(a, name, *, rank, local_rank, world, dist, steps, warmup, with_e2e=True, with_cpu=True, field_cache=None):
+DUMP_ROWS = 250_000  # sampled rows per workload of --dump-outputs: 3 float32 + 5 float64 columns = 13 MB; 52 MB for the 4 default ones
+
+
+def dump_outputs(eng, out_dir, prefix):
+    """The resident particle set after the last timed step: a seeded sample of DUMP_ROWS rows (all rows of smaller sets), in float32
+    (positions) or float64 (time, state, cell index, particle id)."""
+    d = eng.download_all()
+    n = len(d["x"])
+    rows = np.sort(np.random.default_rng(0).choice(n, DUMP_ROWS, replace=False)) if n > DUMP_ROWS else np.arange(n)
+    os.makedirs(out_dir, exist_ok=True)
+    cols = {"x": np.float32, "y": np.float32, "z": np.float32, "t": np.float64, "state": np.float64, "particle_id": np.float64}
+    for k, dt in cols.items():
+        np.save(os.path.join(out_dir, f"{prefix}_{k}.npy"), d[k][rows].astype(dt))
+    np.save(os.path.join(out_dir, f"{prefix}_ei.npy"), d["ei"][rows, -1].astype(np.float64))
+    np.save(os.path.join(out_dir, f"{prefix}_row.npy"), rows.astype(np.float64))
+
+
+def run_gpu_workload(a, name, *, rank, local_rank, world, dist, steps, warmup, with_e2e=True, with_cpu=True, field_cache=None,
+                     dump_dir=None):
     """Measure one workload on this rank's GPU: device-resident arm, end-to-end arm, and (rank 0, N = 1) the parity sample.
     Returns the dict of the JSON line's workload-specific keys (rank 0) or None."""
     import torch
@@ -607,6 +636,8 @@ def run_gpu_workload(a, name, *, rank, local_rank, world, dist, steps, warmup, w
     value = total_steps / (dev_ms * 1e-3)
     kernel_ms = ksum / steps
     steps_per_launch = psteps / steps
+    if dump_dir and rank == 0:
+        dump_outputs(eng, dump_dir, name)
 
     # ---- end-to-end arm: public API with host arrays; H2D + D2H of the particle SoA every step ----
     e2e = None
@@ -801,8 +832,8 @@ def run_decomposed_bench(a, rank, local_rank, world, dist, workload="c5"):
 
 
 def decomposed_bitexact_check(rank, local_rank, world, dist, n=200_000, transport="p2p"):
-    """Mode D over NCCL against ONE GPU, bit for bit (scripts/decomposed_check.py inside the bench, so that the driver's
-    multi-GPU box exercises it): a small field cut into `world` slabs, many slab crossings."""
+    """Mode D over NCCL against ONE GPU, bit for bit (scripts/decomposed_check.py inside the bench, so that every
+    multi-GPU bench run exercises it): a small field cut into `world` slabs, many slab crossings."""
     import parcels_b200 as pb
     from parcels_b200 import distributed as D
     from parcels_b200.particle import create_particle_data
@@ -840,9 +871,15 @@ def decomposed_bitexact_check(rank, local_rank, world, dist, n=200_000, transpor
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--steps", type=int, default=20,
+                    help="timed steps of the main workload's device-resident arm (`value`, `steps` of the line); the blocks under "
+                         "`extra` time max(3, min(steps, 5)), the end-to-end arm min(steps, 5) for sets above 2e6 particles (each "
+                         "of its steps holds a pinned host copy of the set)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps of each workload, write the particle set its last step computed (rank 0; a "
+                         f"seeded sample of {DUMP_ROWS} rows of larger sets) as DIR/<workload>_<column>.npy")
     ap.add_argument("--workload", default="ns", choices=list(WORKLOADS) + list(C5))
     ap.add_argument("--extras", default=None, help="comma-separated workloads measured as compact blocks under `extra` "
                                                    "(default: c2,c3,c4 with the default workload at N=1, none otherwise)")
@@ -916,11 +953,12 @@ def main():
     cache = {}
     t_main = time.perf_counter()
     main_out = run_gpu_workload(a, name, rank=rank, local_rank=local_rank, world=world, dist=dist, steps=a.steps, warmup=a.warmup,
-                                with_e2e=not a.no_e2e, with_cpu=not a.no_cpu_baseline, field_cache=cache)  # fmt: skip
+                                with_e2e=not a.no_e2e, with_cpu=not a.no_cpu_baseline, field_cache=cache, dump_dir=a.dump_outputs)  # fmt: skip
     extra_out = {}
     for e in extras:
         r = run_gpu_workload(a, e, rank=rank, local_rank=local_rank, world=world, dist=dist, steps=max(3, min(a.steps, 5)),
-                             warmup=max(3, min(a.warmup, 3)), with_e2e=not a.no_e2e, with_cpu=not a.no_cpu_baseline, field_cache=cache)  # fmt: skip
+                             warmup=max(3, min(a.warmup, 3)), with_e2e=not a.no_e2e, with_cpu=not a.no_cpu_baseline, field_cache=cache,
+                             dump_dir=a.dump_outputs)  # fmt: skip
         if r is not None:
             r["config"] = config_block(e, WORKLOADS[e], a.particles or WORKLOADS[e]["n"])
             extra_out[e] = r

@@ -1,4 +1,4 @@
-/* parcels_b200.h -- C-ABI of libparcels_b200.so: the B200-native replacement for the hot path
+/* parcels_b200.h -- C-ABI of libparcels_b200.so: the H100 (sm_90a) replacement for the hot path
  * ParticleSet.execute(AdvectionRK4 | AdvectionRK4_3D | AdvectionEE | AdvectionRK2[_3D] [+ DiffusionUniformKh]
  *                     | AdvectionRK45 | AdvectionDiffusionM1 | AdvectionDiffusionEM   [+ delete-on-error handler])
  * on rectilinear A-grids (XLinear_Velocity, XFreeslip, XPartialslip, nearest node) and rectilinear / curvilinear

@@ -132,7 +132,7 @@ inline cudaError_t cudaSetDevice(int) { return hs_enabled() ? cudaSuccess : cuda
 inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp* p, int) {
     std::memset(p, 0, sizeof(*p));
     std::snprintf(p->name, sizeof(p->name), "hostsim (kernel sources compiled for the CPU; tests only)");
-    p->major = 10; p->minor = 0;  // the engine insists on sm_100: the simulated device claims to be one
+    p->major = 9; p->minor = 0;  // the engine insists on sm_90: the simulated device claims to be one
     p->multiProcessorCount = 1;
     return cudaSuccess;
 }

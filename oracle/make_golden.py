@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE ONLY -- generates the committed fixtures under ``tests/golden/``.
 
-Run in the build container (needs ``/root/reference``):  ``python -m oracle.make_golden``
+Run where the reference tree is present (``PARCELS_REFERENCE_SRC``, see ``oracle/ref_harness.py``):  ``python -m oracle.make_golden``
 
 Fixtures produced
 -----------------
@@ -29,10 +29,12 @@ import sys
 
 import numpy as np
 
+from oracle.ref_harness import REFERENCE_SRC
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 GOLDEN = os.path.join(ROOT, "tests", "golden")
-REF_TESTDATA = "/root/reference/tests/test_data"
+REF_TESTDATA = os.path.join(os.path.dirname(os.path.dirname(REFERENCE_SRC)), "tests", "test_data")
 
 
 # ----------------------------------------------------------------------------------------------
@@ -242,6 +244,59 @@ def make_ref_cases(only=None):
         out[f"{name}/error"] = np.array(err)
         print(f"{name}: n_out={len(ps._data['x'])} err={err!r} states={np.unique(ps._data['state'])}")
     np.savez_compressed(os.path.join(GOLDEN, "ref_cases.npz"), **out)
+
+
+def make_selection_golden():
+    """The reference's own output-row rule (_core/particlefile.py ``_to_write_particles``) on 20 seeded random draws: times with
+    NaNs, both signs of dt -> ``tests/golden/selection_rule.npz``."""
+    from oracle import ref_harness as rh
+
+    rh.install()
+    from parcels._core.particlefile import _to_write_particles
+
+    rng = np.random.default_rng(5)
+    out = {}
+    for i in range(20):
+        n = 500
+        t = np.round(rng.uniform(0, 100, n))
+        t[rng.uniform(size=n) < 0.1] = np.nan
+        dt = np.full(n, rng.choice([-7.0, 3.0, 10.0]))
+        tout = float(np.round(rng.uniform(0, 100)))
+        out.update({f"{i}/t": t, f"{i}/dt": dt, f"{i}/tout": np.array(tout),
+                    f"{i}/rows": _to_write_particles({"t": t, "dt": dt, "particle_id": np.arange(n)}, tout)})  # fmt: skip
+    np.savez_compressed(os.path.join(GOLDEN, "selection_rule.npz"), **out)
+
+
+REFERENCE_FUZZ_CASES = 140
+REFERENCE_FUZZ_COLUMNS = ("particle_id", "state", "t", "ei", "dt", "x", "y", "z")
+
+
+def make_reference_fuzz_golden(seed=2026):
+    """The reference's own ``ParticleSet.execute`` on REFERENCE_FUZZ_CASES random trajectory configurations (the generators of
+    scripts/fuzz_hostsim.py: rectilinear dtypes / meshes / schemes / interpolators, every seventh a random curvilinear C-grid,
+    boundary releases, non-finite positions, releases outside the time interval) -> ``tests/golden/reference_fuzz.npz``: each
+    case's spec, its release arrays, the reference's particle data afterwards and the class of what it raised.
+    scripts/replay_reference_fuzz.py runs the same cases through the engine."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    sys.path.insert(0, os.path.join(ROOT, "scripts"))
+    import cases
+    from fuzz_hostsim import inject_boundary_cases, random_curv_spec, random_spec
+    from fuzz_install_vs_reference import run
+
+    rng = np.random.default_rng(seed)
+    out = {}
+    for k in range(REFERENCE_FUZZ_CASES):
+        spec = random_curv_spec(rng) if k % 7 == 3 else random_spec(rng)
+        if spec["kind"] == "curv" and rng.random() < 0.4:
+            spec["interp"] = "linear"  # XLinear_Velocity behind the curvilinear search
+        c = cases.build(spec)
+        inject_boundary_cases(rng, spec, c)
+        ps, err = run(c, spec, False, False)
+        out[f"{k}/spec"] = np.array(json.dumps(spec))
+        out.update({f"{k}/in_{key}": np.asarray(c[key]) for key in "xyzt"})
+        out.update({f"{k}/{key}": ps._data[key] for key in REFERENCE_FUZZ_COLUMNS})
+        out[f"{k}/error"] = np.array(err.rsplit(".", 1)[-1])
+    np.savez_compressed(os.path.join(GOLDEN, "reference_fuzz.npz"), **out)
 
 
 OUTPUT_CASES = {"delayed_partial": 300.0, "flat_f32c_f64d": 30.0, "backward": None}
@@ -559,6 +614,12 @@ if __name__ == "__main__":
         sys.path.insert(0, os.path.join(ROOT, "tests"))
         make_advdiff_golden(only=set(sys.argv[2:]))
         sys.exit(0)
+    if len(sys.argv) > 1 and sys.argv[1] == "reference_fuzz":
+        make_reference_fuzz_golden()
+        sys.exit(0)
+    if len(sys.argv) > 1 and sys.argv[1] == "selection_rule":
+        make_selection_golden()
+        sys.exit(0)
     if len(sys.argv) > 2 and sys.argv[1] == "ref_cases":
         make_ref_cases(only=set(sys.argv[2:]))
         sys.exit(0)
@@ -568,6 +629,8 @@ if __name__ == "__main__":
     make_v3("nearest", "v3_jit_nearest.npz")
     make_ref_cases()
     make_output_golden()
+    make_selection_golden()
+    make_reference_fuzz_golden()
     make_scalar_golden()
     make_scalar_curv_golden()
     make_rk45_golden()

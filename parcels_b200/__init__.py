@@ -1,7 +1,7 @@
-"""parcels_b200 -- B200-native Lagrangian particle advection behind the Parcels v4 API.
+"""parcels_b200 -- Lagrangian particle advection on the H100 behind the Parcels v4 API.
 
 ``ParticleSet.execute([AdvectionRK4 | AdvectionRK4_3D | ...], dt=, runtime=|endtime=)`` runs the
-whole per-particle time loop in hand-written sm_100a CUDA (``csrc/engine.cu``) through the C-ABI
+whole per-particle time loop in hand-written sm_90a CUDA (``csrc/engine.cu``) through the C-ABI
 ``include/parcels_b200.h`` (ctypes).  There is no CPU implementation in this package.
 """
 

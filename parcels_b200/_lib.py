@@ -1,6 +1,6 @@
 """ctypes binding of ``libparcels_b200.so`` (C-ABI: ``include/parcels_b200.h``).
 
-The shared library is built in-tree by ``parcels_b200.build`` (nvcc, sm_100a only).  If it is
+The shared library is built in-tree by ``parcels_b200.build`` (nvcc, sm_90a only).  If it is
 missing or a symbol is absent, importing the engine fails loudly -- there is no fallback.
 """
 
@@ -183,7 +183,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise EngineError(
             f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a). parcels_b200 has no CPU fallback."
+            "(nvcc, sm_90a). parcels_b200 has no CPU fallback."
         )
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in SYMBOLS.items():

@@ -1,4 +1,4 @@
-"""In-tree build of ``libparcels_b200.so`` with nvcc for sm_100a (no other target, no fallback)."""
+"""In-tree build of ``libparcels_b200.so`` with nvcc for sm_90a (H100; no other target, no fallback)."""
 
 from __future__ import annotations
 
@@ -8,8 +8,9 @@ import subprocess
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SOURCES = ["engine.cu", "afast.cu", "agrid.cu", "aslip.cu", "rk45.cu", "advdiff.cu", "hashbuild.cu", "cgrid.cu", "curva.cu"]  # one translation unit per kernel family: compiled in parallel
-# Per-source tuning (measured on B200, profiles/README.md): the A-grid kernel runs best with its corner
-# cache in shared memory (float64 copies on float64 grids) and <= 128 registers (4 blocks of 128 threads per SM).
+# Per-source tuning: the A-grid kernels keep their corner cache in shared memory (float64 copies on float64 grids); PB_MINBLOCKS
+# caps the registers through the blocks that must be resident per SM (64 K registers per SM on the H100): 4 blocks of 128 threads
+# allow 128 registers (agrid / aslip), 3 allow 170 (afast, whose hot loop needs 168; rk45, cgrid, curva).
 EXTRA_FLAGS = {"afast.cu": ["-DPB_BLOCK=128", "-DPB_MINBLOCKS=3", "-DPB_SMEM_CACHE"], "agrid.cu": ["-DPB_MINBLOCKS=4", "-DPB_SMEM_CACHE"], "aslip.cu": ["-DPB_MINBLOCKS=4", "-DPB_SMEM_CACHE"],
                "rk45.cu": ["-DPB_MINBLOCKS=3", "-DPB_SMEM_CACHE"], "advdiff.cu": ["-DPB_SMEM_CACHE"],
                "cgrid.cu": ["-DPB_MINBLOCKS=3"], "curva.cu": ["-DPB_MINBLOCKS=3"]}  # fmt: skip
@@ -19,7 +20,7 @@ HEADER = os.path.join(os.path.dirname(HERE), "include", "parcels_b200.h")
 
 NVCC_FLAGS = [
     "-O3", "-std=c++17",
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo",
     "-fmad=false",  # no FMA contraction: arithmetic must round exactly like the reference's NumPy ops
     "-Xcompiler", "-fPIC",
@@ -54,7 +55,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         if verbose:
             print(err)
         objs.append(obj)
-    cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", OUT, *objs, "-ldl"]
+    cmd = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", OUT, *objs, "-ldl"]
     res = subprocess.run(cmd, capture_output=True, text=True)
     if res.returncode != 0:
         raise RuntimeError(f"link failed:\n{' '.join(cmd)}\n{res.stdout}\n{res.stderr}")

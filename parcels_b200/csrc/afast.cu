@@ -19,14 +19,13 @@
 //    interleave_kernel below): 16 x 16-byte loads instead of 48 scattered 4-byte ones, a fifth of the DRAM traffic.
 //  * On a cell miss the two neighbouring cells are tried before the full binary search (a particle crosses one face at a time).
 //
-// TWO SCHEDULES of the same evaluation (template parameter SCHED; the 32 KB L1.5 instruction cache decides -- profiles/README.md
-// r02g-r02n, config 2 / 1/12 deg workload / fused diffusion in ms):
+// TWO SCHEDULES of the same evaluation (template parameter SCHED; the instruction cache decides):
 //   SCHED 2 (advection-only lists): a TWO-stage loop body -- a stage that reuses the T-lerped block and one that renews it, the
-//     choice a compile-time constant, run twice per step, both side-path copies inline: 13.9 / 177 / (318).
-//   SCHED 1 (lists with DiffusionUniformKh): ONE evaluation site in a four-trip stage loop, "renew" a run-time flag: 15.8 / 198 / 212
+//     choice a compile-time constant, run twice per step, both side-path copies inline.
+//   SCHED 1 (lists with DiffusionUniformKh): ONE evaluation site in a four-trip stage loop, "renew" a run-time flag
 //     -- next to the Philox / Box-Muller block only one copy of the hit and side paths fits the cache.
-//   Tried and measured slower: all four stages written out (17.0 / 259 / 396: 5000 SASS instructions, `stall_no_inst` on top), the
-//   side path or the diffusion increment out of line (208 / 342: every call spills the hit path's live registers).
+//   Tried and measured slower: all four stages written out (5000 SASS instructions: instruction-fetch stalls), the
+//   side path or the diffusion increment out of line (every call spills the hit path's live registers).
 #include <cmath>
 
 #include "agrid.cuh"
@@ -225,7 +224,7 @@ struct AFastPolicy {
 
     // ---------------- side path: searches, states, refill; special samples are finished here ----------------
     // Inline at every evaluation site (out of line it costs the spill / reload of the hit path's live registers at every trip:
-    // measured, r02l).  Reads and rewrites the lane's cells / reciprocals / indices / raw block in shared memory; what the caller
+    // measured).  Reads and rewrites the lane's cells / reciprocals / indices / raw block in shared memory; what the caller
     // has in registers comes in as arguments and goes back through `out`.
     __device__ static __forceinline__
     void side_path(const AdvectParams* pp, float4* raw, int k, double ts, double zs, double ys, double xs, int state, SideResult* out) {

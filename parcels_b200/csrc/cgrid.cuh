@@ -32,8 +32,8 @@ static __device__ __noinline__ float cosf_ool(float x) { return cosf(x); }
 static __device__ __noinline__ float sinf_ool(float x) { return sinf(x); }
 __device__ __forceinline__ float cosx(float x) { return cosf_ool(x); }
 __device__ __forceinline__ double cosx(double x) { return cos_np(x); }  // (a latitude: common.cuh's polynomial, inline)
-// Per-sample trigonometry of the curvilinear search (ncu, profiles/README.md r02f: the out-of-line cos / sin above were 33 % of the
-// executed instructions of config 3 -- 24 + 8 calls of ~70 instructions per warp and step).  The query's unit vector needs
+// Per-sample trigonometry of the curvilinear search (out-of-line cos / sin like the ones above would be 24 + 8 calls of ~70
+// instructions per warp and step on config 3).  The query's unit vector needs
 // sin / cos of a LATITUDE (|x| <= pi/2: one odd polynomial each, like cos_np) and of a LONGITUDE (|x| <= 4 pi: one shared
 // quadrant reduction + the two fdlibm kernel polynomials on [-pi/4, pi/4]); <= 2 ulp like CUDA's own, anything outside those
 // ranges takes sincos().  The one-time per-cell table (project_cell) keeps CUDA's sin / cos.
@@ -715,7 +715,7 @@ struct CurvPolicy {
             }
             if (!nb) {
                 // (inline on purpose: out of line -- 0.03 queries per warp-step, ~350 instructions -- the call spills the caller's live
-                //  registers: 188.7 vs 160.8 ms on config 3, profiles/README.md r02l)
+                //  registers)
                 hash_query(g, e, q, xy_f32 ? isfinite((float)x) && isfinite((float)y) : isfinite(x) && isfinite(y), qx, qy, qz, yi, xi, xsi, eta);
             }
         }

@@ -1,4 +1,4 @@
-// engine.cu -- libparcels_b200.so: hand-written sm_100a CUDA for the Parcels hot path
+// engine.cu -- libparcels_b200.so: hand-written sm_90a CUDA for the Parcels hot path
 //   ParticleSet.execute(AdvectionRK4 | AdvectionRK4_3D | AdvectionEE | AdvectionRK2[_3D]
 //                       [+ DiffusionUniformKh] [+ delete-on-error])
 // behind the C-ABI declared in include/parcels_b200.h.
@@ -15,9 +15,9 @@
 //    f32/f64 grid coordinates and data, f64 time) operation by operation, with FMA contraction OFF
 //    (-fmad=false), so cell indices are bit-exact and trajectories agree to the last f32 ulp
 //    (transcendentals aside);
-//  * no tensor cores: this is a gather + fp64 lerp path, there is no contraction to map on tcgen05.
+//  * no tensor cores: this is a gather + fp64 lerp path, there is no contraction to map on wgmma.
 //
-// This file is compiled ONLY for sm_100a.  There is no CPU fallback anywhere in the product.
+// This file is compiled ONLY for sm_90a (H100).  There is no CPU fallback anywhere in the product.
 
 #include <cuda_runtime.h>
 
@@ -388,7 +388,8 @@ int32_t pb_engine_create(int32_t device, pb_engine** out) {
     CK(cudaSetDevice(device));
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, device));
-    if (prop.major < 10) return fail(PB_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_100a only", device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0)  // sm_90a code loads on compute capability 9.0 only
+        return fail(PB_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", device, prop.major, prop.minor);
     pb_engine* e = new pb_engine();
     e->device = device;
     CK(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
@@ -941,17 +942,15 @@ int32_t pb_sample_scalar(pb_engine* e, int32_t slot, int32_t method, int64_t n, 
 // The specialised RK4 kernel (afast.cu) gathers from a node-interleaved {u, v, w, 0} copy of the float32 fields: built here, on
 // the device, the first time an RK4 launch can use it (float64 rectilinear grid, XLinear_Velocity, every level resident).
 #ifndef PB_FAST_DEFAULT_DIFFUSION
-#define PB_FAST_DEFAULT_DIFFUSION 1  // (measured, profiles/README.md r02m / r02n)
+#define PB_FAST_DEFAULT_DIFFUSION 1
 #endif
 static bool fast_kernel_enabled() {
     const char* v = getenv("PB_DISABLE_FAST_KERNEL");  // A/B switch of the parity tests and variant sweeps
     return !(v && v[0] == '1');
 }
 // which schedule of the specialised RK4 kernel (afast.cu): 2 = a two-stage loop body with compile-time renew / reuse, 1 = one
-// evaluation site in a four-trip loop.  Measured (profiles/README.md r02m): advection only 14.2 vs
-// 15.8 ms on config 2 and 180 vs 198 ms on the 1/12 deg workload for schedule 2; with the fused diffusion block the two-stage body
-// overflows the instruction cache (318 ms inline, 342 ms with the increment out of line, against 212 ms): lists with
-// DiffusionUniformKh run schedule 1.  PB_FAST_KERNEL=1|2 forces one.
+// evaluation site in a four-trip loop.  Schedule 2 is the faster one for advection only; with the fused diffusion block the
+// two-stage body overflows the instruction cache: lists with DiffusionUniformKh run schedule 1.  PB_FAST_KERNEL=1|2 forces one.
 static int fast_kernel_version(bool diffusion) {
     const char* v = getenv("PB_FAST_KERNEL");
     if (v && v[0] == '1') return 1;
@@ -1099,8 +1098,8 @@ int32_t pb_advect_host(pb_engine* e, const pb_advect_args* a, int64_t n, const p
     CK(cudaMemcpyAsync(e->d_rep, e->h_rep, sizeof(ReportDev), cudaMemcpyHostToDevice, e->stream));
     CK(cudaEventRecord(e->ev0, e->stream));
     CK(cudaEventRecord(e->pipe_fork, e->stream));
-    // chunks of whole thread blocks; small sets are not cut
-    const long long align = 256 * 148;
+    // chunks of whole waves of 256-thread blocks over the H100's 132 SMs; small sets are not cut
+    const long long align = 256 * 132;
     long long chunks = n_chunks < 1 ? 1 : n_chunks;
     long long per = n > 0 ? ((n + chunks - 1) / chunks + align - 1) / align * align : 0;
     if (per <= 0) per = align;

@@ -96,7 +96,7 @@ class ParticleFile:
         if self._writer is None:
             # Same schema, values and compression as the reference's writer (:155-160).  Dictionary encoding is kept
             # for `t` only (few distinct values per write): attempting it on the float position columns and the
-            # ids is what dominates pyarrow's encode time (3.5x, profiles/README.md) and never pays off there.
+            # ids is what dominates pyarrow's encode time and never pays off there.
             self._writer = pq.ParquetWriter(self.path, self._schema(pclass, fieldset), compression=self._compression,
                                             use_dictionary=["t"])
         if isinstance(t, np.datetime64):

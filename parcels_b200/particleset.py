@@ -433,7 +433,7 @@ class ParticleSet:
         self._host_stale = False
         self.eager_host = False  # True: refresh the host arrays at the end of every execute() (shared-array adapters)
         # > 1: Kernel.execute on host arrays runs as that many pipelined chunks (copies under kernels, pb_advect_host)
-        # (default 8: measured on the B200, profiles/README.md r02 -- copies of one chunk run under the kernels of the others)
+        # (default 8: copies of one chunk run under the kernels of the others)
         self.pipeline_chunks = int(os.environ.get("PB_PIPELINE_CHUNKS", "8"))
         self._n_device = 0
         self._stale_dt = 1.0

@@ -28,5 +28,5 @@ for src in b.SOURCES:
                 print(f"[{tag} {src}]", ln.split("for ")[1][:60], lines[i + 1].strip(), "|", lines[i + 2].strip().replace("ptxas info    : ", ""))
     objs.append(obj)
 out = os.path.join(b.HERE, "lib", f"libparcels_b200_{tag}.so")
-subprocess.run(["nvcc", "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", out, *objs, "-ldl"], check=True)
+subprocess.run(["nvcc", "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", out, *objs, "-ldl"], check=True)
 print(out)

@@ -108,6 +108,53 @@ def inject_boundary_cases(rng, spec, c):
         c["t"] = np.where(rng.random(n) < 0.5, 0.0, later)
 
 
+def compare_with_reference(spec, c, da, ea, db, eb):
+    """Differences of the engine's particle data ``db`` (raised ``eb``) from the reference's ``da`` (raised ``ea``) after the same
+    trajectory case: ids / states / times / cells / dt identical, positions bit-exact on flat meshes and within a few float32 ulp
+    on spherical ones; curvilinear meshes as stated below."""
+    msg = []
+    if ea != eb:
+        msg.append(f"raised {eb!r} vs the reference's {ea!r}")
+    if len(da["x"]) != len(db["x"]):
+        msg.append(f"survivors {len(db['x'])} vs {len(da['x'])}")
+    else:
+        skip_xyz = ea.endswith("OutsideTimeInterval")  # DESIGN.md waiver 2: dx / ei of the aborted step
+        if spec["kind"] == "curv" and spec["mesh"] == "flat":
+            # the reference's flat-mesh bilinear inverse is ill-conditioned on random near-parallelogram cells and changes with
+            # its own batch size (DESIGN.md waiver 6): only who is left, in which state and at what time is compared
+            for key in ("particle_id", "state", "t"):
+                if not np.array_equal(da[key], db[key]):
+                    msg.append(key)
+            return msg
+        if ea.endswith("IndexError"):
+            return []  # the reference's own failure (3-D slip, no particle below the first level: DESIGN.md waiver 1)
+        for key in ("particle_id", "state", "t") + (() if skip_xyz else ("ei", "dt")):
+            if not np.array_equal(da[key], db[key]):
+                msg.append(key)
+        if not skip_xyz:
+            for key in "xyz":
+                floor = 0.01 * float(np.abs(np.asarray(c[key])).max()) or None
+                u = ulp_diff_f32(db[key], da[key], floor=floor)
+                tol = 0 if spec["mesh"] == "flat" else 4
+                if spec["kind"] == "curv":
+                    # curvilinear C-grids (hint + neighbour + spatial-hash search) on SPHERICAL random meshes: cells, states and
+                    # times identical; positions within 1e-4 of a cell -- the set is fresh, so the reference computes its first
+                    # evaluation with float32-TYPED barycentric coordinates (DESIGN.md waiver 4: 1e-7 relative) and the C-grid's
+                    # face discontinuities grow that seed (measured over 300 random meshes: <= 2 float32 ulp with float64
+                    # nodes, <= 11 with float32 nodes, rarely more).  FLAT random meshes: see below.
+                    cell = float(np.abs(np.diff(np.asarray(c["lon"], dtype=np.float64), axis=1)).mean())
+                    if len(da[key]) and float(np.abs(db[key].astype(np.float64) - da[key].astype(np.float64)).max()) > 1e-4 * cell:
+                        msg.append(f"{key}: {float(np.abs(db[key].astype(np.float64) - da[key].astype(np.float64)).max()) / cell:.2e} cells")
+                    continue
+                if spec["mesh"] == "flat" and spec.get("interp") == "cgrid_velocity":
+                    tol = 0.5  # (a batch of exactly one evaluated particle: DESIGN.md waiver 8)
+                if spec["mesh"] == "spherical" and spec.get("interp") == "cgrid_velocity" and spec["cdtype"] == "f4":
+                    tol = 64  # (float32 edge lengths with a float32 cos, main() below)
+                if u.size and u.max() > tol:
+                    msg.append(f"{key}: {u.max():.1f} ulp (tol {tol})")
+    return msg
+
+
 def main():
     argv = [a for a in sys.argv[1:] if not a.startswith("--")]
     n_cases = int(argv[0]) if argv else 100

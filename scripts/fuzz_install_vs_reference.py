@@ -24,7 +24,7 @@ import parcels._core.statuscodes as rcodes  # noqa: E402
 import cases  # noqa: E402
 import parcels_b200 as pb  # noqa: E402
 from engine_run import ulp_diff_f32  # noqa: E402
-from fuzz_hostsim import inject_boundary_cases, random_curv_spec, random_spec  # noqa: E402
+from fuzz_hostsim import compare_with_reference, inject_boundary_cases, random_curv_spec, random_spec  # noqa: E402
 
 warnings.simplefilter("ignore")
 K = rh.kernels()
@@ -339,50 +339,7 @@ def main():
             bad += 1
             continue
         on_engine += b.__dict__.get("_b200_pset") is not None
-        msg = []
-        if ea != eb:
-            msg.append(f"raised {eb!r} vs the reference's {ea!r}")
-        da, db = a._data, b._data
-        if len(da["x"]) != len(db["x"]):
-            msg.append(f"survivors {len(db['x'])} vs {len(da['x'])}")
-        else:
-            skip_xyz = ea.endswith("OutsideTimeInterval")  # DESIGN.md waiver 2: dx / ei of the aborted step
-            if spec["kind"] == "curv" and spec["mesh"] == "flat":
-                # the reference's flat-mesh bilinear inverse is ill-conditioned on random near-parallelogram cells and changes with
-                # its own batch size (DESIGN.md waiver 6): only who is left, in which state and at what time is compared
-                for key in ("particle_id", "state", "t"):
-                    if not np.array_equal(da[key], db[key]):
-                        msg.append(key)
-                if msg:
-                    bad += 1
-                    print(f"[{k}] MISMATCH {'; '.join(msg)}  (token={token})\n    spec={spec}")
-                continue
-            if ea.endswith("IndexError"):
-                continue  # the reference's own failure (3-D slip, no particle below the first level: DESIGN.md waiver 1)
-            for key in ("particle_id", "state", "t") + (() if skip_xyz else ("ei", "dt")):
-                if not np.array_equal(da[key], db[key]):
-                    msg.append(key)
-            if not skip_xyz:
-                for key in "xyz":
-                    floor = 0.01 * float(np.abs(np.asarray(c[key])).max()) or None
-                    u = ulp_diff_f32(db[key], da[key], floor=floor)
-                    tol = 0 if spec["mesh"] == "flat" else 4
-                    if spec["kind"] == "curv":
-                        # curvilinear C-grids (hint + neighbour + spatial-hash search) on SPHERICAL random meshes: cells, states and
-                        # times identical; positions within 1e-4 of a cell -- the set is fresh, so the reference computes its first
-                        # evaluation with float32-TYPED barycentric coordinates (DESIGN.md waiver 4: 1e-7 relative) and the C-grid's
-                        # face discontinuities grow that seed (measured over 300 random meshes: <= 2 float32 ulp with float64
-                        # nodes, <= 11 with float32 nodes, rarely more).  FLAT random meshes: see below.
-                        cell = float(np.abs(np.diff(np.asarray(c["lon"], dtype=np.float64), axis=1)).mean())
-                        if len(da[key]) and float(np.abs(db[key].astype(np.float64) - da[key].astype(np.float64)).max()) > 1e-4 * cell:
-                            msg.append(f"{key}: {float(np.abs(db[key].astype(np.float64) - da[key].astype(np.float64)).max()) / cell:.2e} cells")
-                        continue
-                    if spec["mesh"] == "flat" and spec.get("interp") == "cgrid_velocity":
-                        tol = 0.5  # (a batch of exactly one evaluated particle: see rk45_case)
-                    if spec["mesh"] == "spherical" and spec.get("interp") == "cgrid_velocity" and spec["cdtype"] == "f4":
-                        tol = 64  # (float32 edge lengths with a float32 cos, scripts/fuzz_hostsim.py)
-                    if u.size and u.max() > tol:
-                        msg.append(f"{key}: {u.max():.1f} ulp (tol {tol})")
+        msg = compare_with_reference(spec, c, a._data, ea, b._data, eb)
         if msg:
             bad += 1
             print(f"[{k}] MISMATCH {'; '.join(msg)}  (token={token})\n    spec={spec}")

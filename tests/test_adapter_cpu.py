@@ -1,4 +1,4 @@
-"""CPU test (build container only): the adapter reads a live reference FieldSet correctly."""
+"""CPU test (needs the reference's own Python package, oracle/ref_harness.py): the adapter reads a live reference FieldSet correctly."""
 
 import numpy as np
 import pytest
@@ -6,7 +6,7 @@ import pytest
 from oracle import ref_harness as rh
 from oracle_run import load_case
 
-pytestmark = pytest.mark.skipif(not rh.reference_available(), reason="/root/reference not present")
+pytestmark = pytest.mark.skipif(not rh.reference_available(), reason="the reference's own Python package is not importable (PARCELS_REFERENCE_SRC)")
 
 
 def test_from_parcels_reads_reference_fieldset():

@@ -2,8 +2,8 @@
 CPU oracle fed the engine's own Philox stream: ids, states, times, surviving set and cell indices bit-exact; positions
 bit-exact on flat meshes, <= 4 float32 ulp on spherical meshes (CUDA cos / cosf vs glibc) -- ulps of max(|x|, D), D = the
 largest displacement any particle made in the run: the longitudes of these cases cross zero, where a 1-ulp rounding flip made
-while the particle was at |x| ~ 0.4 deg is 30 ulps of a final x = 0.02 deg (measured on the B200: every particle agrees to
-<= 3 ulp except the one that ends next to zero; and with the oracle alone: perturbing its float32 cos by 1 ulp moves a particle
+while the particle was at |x| ~ 0.4 deg is 30 ulps of a final x = 0.02 deg (every particle agrees to <= 3 ulp except the one
+that ends next to zero; and with the oracle alone: perturbing its float32 cos by 1 ulp moves a particle
 ending at x = -0.0008 by 150 of ITS ulps).  The oracle itself is pinned to
 the reference's outputs with the reference's RNG (tests/test_advdiff_cpu.py).  Statistical check against the reference's
 own test (tests/test_diffusion.py:49-81): zero mean, zonal skew > meridional skew on a field with a zonal Kh gradient."""

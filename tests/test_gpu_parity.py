@@ -1,4 +1,4 @@
-"""GPU parity tests (-m gpu): the product path (parcels_b200 -> ctypes C-ABI -> sm_100a CUDA)
+"""GPU parity tests (-m gpu): the product path (parcels_b200 -> ctypes C-ABI -> sm_90a CUDA)
 against the CPU oracle on the same seeded inputs, and against the committed outputs of the
 reference itself (tests/golden/).
 

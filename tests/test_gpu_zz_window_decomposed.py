@@ -1,6 +1,6 @@
 """GPU test of time-slab streaming UNDER mode D (DESIGN.md 7b): 2 ranks on cuda:0, each with 2 of 6 time levels of its X-slab
-resident, windows slid in lock-step -- bit-exact against the undecomposed run that keeps every level resident.  (Written after the
-round's last B200 run: the host simulation has run it, tests/test_hostsim_cpu.py; the file sorts last on purpose.)"""
+resident, windows slid in lock-step -- bit-exact against the undecomposed run that keeps every level resident.  (The host
+simulation runs it too, tests/test_hostsim_cpu.py; the file sorts last on purpose.)"""
 
 import os
 import subprocess

@@ -4,7 +4,7 @@
 This checks the LOGIC of the CUDA sources -- state machine, searches, interpolation arithmetic, error / delete / replay
 handling, output selection, hash build, host bindings -- against the oracle and the reference's golden outputs on machines
 without a GPU.  It is test infrastructure: the product never loads the simulation (it needs PB_LIB pointing at it AND
-PB_HOSTSIM_TEST=1), and the real parity statement is `pytest -m gpu` on the B200."""
+PB_HOSTSIM_TEST=1), and the real parity statement is `pytest -m gpu` on the H100."""
 
 import os
 import shutil
@@ -200,6 +200,19 @@ def test_nan_node_on_the_device_side_hash_build_and_query():
     assert r.returncode == 0 and "PASS nan node" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]
 
 
+def test_random_configurations_against_the_references_stored_outputs():
+    """140 random trajectory configurations (scripts/fuzz_hostsim.py's generators: dtypes, meshes, 2-D / 3-D, five schemes, five
+    interpolators, random curvilinear C-grids, boundary releases, non-finite coordinates, releases outside the time interval) through
+    the public API, against what the reference's own ParticleSet.execute produced on them (tests/golden/reference_fuzz.npz)."""
+    from oracle.hostsim import build as hb
+
+    lib = hb.build()
+    r = subprocess.run([sys.executable, os.path.join(ROOT, "scripts", "replay_reference_fuzz.py")], capture_output=True, text=True,
+                       timeout=900, cwd=ROOT, env=_env(lib))  # fmt: skip
+    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-2000:]
+    assert r.stdout.strip().endswith("140 cases against the reference's stored outputs, 0 with differences"), r.stdout[-3000:]
+
+
 def _bench_line(stdout):
     import json
 
@@ -208,14 +221,18 @@ def _bench_line(stdout):
     return json.loads(lines[0])
 
 
-def test_bench_control_flow_single_rank():
+def test_bench_control_flow_single_rank(tmp_path):
     """bench.py's N = 1 flow on the simulated device (scripts/bench_hostsim.py: torch.cuda entry points stubbed, numbers
-    meaningless): the arms run, the line carries every key of the contract, the parity sample agrees with the oracle."""
+    meaningless): the arms run, the line carries every key of the contract, the parity sample agrees with the oracle, and
+    --dump-outputs writes the particle set of the last timed step."""
+    import numpy as np
+
     from oracle.hostsim import build as hb
 
     lib = hb.build()
+    dump = tmp_path / "dump"
     cmd = [sys.executable, os.path.join(ROOT, "scripts", "bench_hostsim.py"), "--workload", "c2_small", "--particles", "1500", "--steps", "3",
-           "--warmup", "3", "--extras", "c3_small"]  # fmt: skip
+           "--warmup", "3", "--extras", "c3_small", "--dump-outputs", str(dump)]  # fmt: skip
     r = subprocess.run(cmd, capture_output=True, text=True, timeout=900, cwd=ROOT, env=_env(lib))
     assert r.returncode == 0, r.stdout[-1500:] + r.stderr[-2500:]
     d = _bench_line(r.stdout)
@@ -227,6 +244,22 @@ def test_bench_control_flow_single_rank():
     assert set(d["roofline"]) >= {"bound", "achieved", "peak", "unit", "frac", "traffic"}
     assert d["parity_sample"]["ok"] and d["extra"]["c3_small"]["parity_sample"]["ok"]
     assert d["cpu_baseline"]["kind"] == "port" and d["cpu_baseline"]["cores"] == 1
+    for name in ("c3_small", "c2_small"):
+        cols = {k: np.load(dump / f"{name}_{k}.npy") for k in ("x", "y", "z", "t", "state", "ei", "particle_id", "row")}
+        assert all(v.shape == (1500,) and v.dtype in (np.float32, np.float64) for v in cols.values())
+        assert np.array_equal(cols["particle_id"], np.arange(1500))
+    # what was dumped is what the pass computed: the oracle advects the same 1500 particles of c2_small (bench seeds rank 0 with 1)
+    import bench
+    from engine_run import ulp_diff_f32
+
+    w = bench.WORKLOADS["c2_small"]
+    field = w["field"](**w["fkw"])
+    pd, _, _ = bench._oracle_pass("c2_small", w, field, w["particles"](field, 1500, 1))
+    live = pd["particle_id"]
+    assert len(live) > 0 and np.all(cols["state"][np.setdiff1d(np.arange(1500), live)] != 0)  # the rest were deleted
+    assert np.array_equal(cols["t"][live], pd["t"]) and np.array_equal(cols["ei"][live], pd["ei"][:, -1])
+    for k in "xyz":
+        assert ulp_diff_f32(cols[k][live], pd[k], floor=0.05).max() <= w["ulp"], k
 
 
 def test_bench_control_flow_two_ranks_and_the_mode_d_watchdog():

@@ -1,4 +1,4 @@
-"""CPU (build container: needs /root/reference): ``parcels_b200.install()`` patches the reference's ``Kernel.execute`` so that an
+"""CPU (needs the reference's own Python package, oracle/ref_harness.py): ``parcels_b200.install()`` patches the reference's ``Kernel.execute`` so that an
 unmodified reference script -- its own ``ParticleSet``, ``ParticleSet.execute``, kernel functions, exceptions -- runs its inner
 loop on the engine.  The engine here is the host simulation of the kernel sources (oracle/hostsim); tests/install_run.py does the
 same comparison on a real GPU when the reference travels there."""
@@ -13,7 +13,7 @@ import pytest
 from oracle import ref_harness as rh
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-pytestmark = pytest.mark.skipif(not rh.reference_available(), reason="/root/reference not present")
+pytestmark = pytest.mark.skipif(not rh.reference_available(), reason="the reference's own Python package is not importable (PARCELS_REFERENCE_SRC)")
 
 
 @pytest.fixture(scope="module")
@@ -62,7 +62,8 @@ def test_random_configurations_against_the_reference_itself():
     """140 random configurations -- mostly rectilinear (the generator of scripts/fuzz_hostsim.py: dtypes, meshes, 2-D / 3-D, five schemes, five
     interpolators, boundary releases, non-finite coordinates, releases outside the time interval, with and without an error handler)
     through the reference's own ParticleSet.execute, untouched and with install(): identical data, same exception classes
-    (scripts/fuzz_install_vs_reference.py) -- the engine against the REFERENCE, not against the oracle."""
+    (scripts/fuzz_install_vs_reference.py) -- the engine against the REFERENCE, not against the oracle.  The reference's outputs on 140
+    such configurations are stored too: tests/test_hostsim_cpu.py replays them where the reference is absent."""
     from oracle.hostsim import build as hb
 
     env = dict(os.environ, PB_LIB=hb.build(), PB_HOSTSIM_TEST="1", PYTHONPATH=os.pathsep.join([ROOT, os.path.join(ROOT, "tests")]))
