@@ -404,6 +404,21 @@ int32_t pb_delete_view_outside_time(pb_engine* e, double dt, double endtime);
 int32_t pb_debug_normals(pb_engine* e, uint64_t seed, uint64_t rng_call, int64_t iter, int64_t n,
                          const int64_t* particle_id, double* out);
 
+/* Pure helper used by tests: the hand-written math primitives of the kernels (the same inline functions, not copies),
+ * evaluated ON THE DEVICE element by element.  out = 2 doubles per element:
+ *   PB_MATH_COS_NP                cos_np(a[i]), 0                  (common.cuh: cos of a latitude in radians)
+ *   PB_MATH_SIN_LAT               sin_lat(a[i]), 0                 (cgrid.cuh: sin of a latitude in radians)
+ *   PB_MATH_SINCOS_LON            sin, cos of sincos_lon(a[i])     (cgrid.cuh: of a longitude in radians)
+ *   PB_MATH_DIV_BY_CACHED         div_by_cached(a[i], b[i], r), r  (common.cuh; r = 1.0 / b[i] computed on the device)
+ *   PB_MATH_DIV_BY_CACHED_GUARDED div_by_cached_guarded(a[i], b[i], r), r
+ *   PB_MATH_BOX_MULLER_F32        zx, zy of box_muller_f32((uint32_t)a[i], (uint32_t)b[i])  (the two Philox words)
+ * b may be NULL for the first three. */
+enum pb_math_op {
+    PB_MATH_COS_NP = 0, PB_MATH_SIN_LAT = 1, PB_MATH_SINCOS_LON = 2, PB_MATH_DIV_BY_CACHED = 3, PB_MATH_DIV_BY_CACHED_GUARDED = 4,
+    PB_MATH_BOX_MULLER_F32 = 5
+};
+int32_t pb_debug_math(pb_engine* e, int32_t op, int64_t n, const double* a, const double* b, double* out);
+
 /* ---- host-side passes of Kernel.execute / ParticleSet.execute over the particle columns, multi-threaded ----------------
  * The reference makes a few whole-column passes per call on the host: `pset._data["dt"][:] = dt` (_core/particleset.py:405,
  * _core/kernel.py:225-226), `particle_release_times.min() / .max()` (_core/particleset.py:541-544), `state[:] = Evaluate`

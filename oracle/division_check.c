@@ -2,6 +2,9 @@
  * (parcels_b200/csrc/common.cuh div_by_cached): q = a r, two residual corrections with r = RN(1 / b), against the division
  * itself, on bcoord-like operands, random mantissas, the two constant divisors of the hot path (deg2m = 111120, 6) and quotients
  * built next to rounding midpoints.  tests/test_oracle_c.py builds and runs it (gcc -O2 -mfma -ffp-contract=off).
+ * The primary check is tests/test_gpu_math.py, which runs the device function itself (pb_debug_math) on the same distributions;
+ * this host copy is the larger stress run. */
+/*
  * Prints "n=... bad3=... bad5=..." (bad3: a single correction step, for reference); exit status 1 when bad5 != 0. */
 #include <math.h>
 #include <stdio.h>

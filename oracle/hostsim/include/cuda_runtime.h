@@ -84,12 +84,13 @@ inline void sincospi(double x, double* s, double* c) {  // exact reduction to [-
     *s = std::sin(3.14159265358979323846 * r);
     *c = std::cos(3.14159265358979323846 * r);
 }
+// exact reduction in half-turns to an argument where the result is not small, libm in double, one rounding to float: within
+// CUDA's documented 1 ulp (exact zeros at the integers and half-integers, like CUDA's)
 inline void sincospif(float x, float* s, float* c) {
-    float r = std::fmod(x, 2.0f);
-    if (r > 1.0f) r -= 2.0f;
-    if (r < -1.0f) r += 2.0f;
-    *s = std::sin(3.14159265358979323846f * r);
-    *c = std::cos(3.14159265358979323846f * r);
+    const double r = std::remainder((double)x, 2.0);  // [-1, 1], exact
+    const double a = std::fabs(r);
+    *s = (float)std::copysign(std::sin(3.14159265358979323846 * std::min(a, 1.0 - a)), r);  // 1 - a: exact where it is the min
+    *c = (float)(a < 0.25 ? std::cos(3.14159265358979323846 * a) : std::sin(3.14159265358979323846 * (0.5 - a)));  // 0.5 - a: exact
 }
 using std::isfinite;
 // CUDA's min / max accept mixed integer types

@@ -160,6 +160,7 @@ SYMBOLS = {
     "pb_flag_view_outside_time": (C.c_int32, [_P, C.c_double, C.c_double]),
     "pb_delete_view_outside_time": (C.c_int32, [_P, C.c_double, C.c_double]),
     "pb_debug_normals": (C.c_int32, [_P, C.c_uint64, C.c_uint64, C.c_int64, C.c_int64, _P, _P]),
+    "pb_debug_math": (C.c_int32, [_P, C.c_int32, C.c_int64, _P, _P, _P]),
     "pb_host_fill_f64": (C.c_int32, [_P, C.c_int64, C.c_double]),
     "pb_host_fill_i32": (C.c_int32, [_P, C.c_int64, C.c_int32]),
     "pb_host_min_max_f64": (C.c_int32, [_P, C.c_int64, _P, _P, _P]),

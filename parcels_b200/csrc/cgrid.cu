@@ -83,3 +83,25 @@ cudaError_t launch_sample_cgrid(const SampleParams& p, bool coord_f64, bool data
     if (coord_f64) return data_f64 ? sample_ad<double, double>(p, nc, s) : sample_ad<double, float>(p, nc, s);
     return data_f64 ? sample_ad<float, double>(p, nc, s) : sample_ad<float, float>(p, nc, s);
 }
+
+// pb_debug_math: the math primitives the kernels call, one element per lane (here because sin_lat / sincos_lon are cgrid.cuh's)
+__global__ void debug_math_kernel(int op, long long n, const double* a, const double* b, double* out) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const double x = a[i];
+    double o0 = 0.0, o1 = 0.0;
+    switch (op) {
+        case PB_MATH_COS_NP: o0 = cos_np(x); break;
+        case PB_MATH_SIN_LAT: o0 = sin_lat(x); break;
+        case PB_MATH_SINCOS_LON: sincos_lon(x, o0, o1); break;
+        case PB_MATH_DIV_BY_CACHED: o1 = 1.0 / b[i]; o0 = div_by_cached(x, b[i], o1); break;
+        case PB_MATH_DIV_BY_CACHED_GUARDED: o1 = 1.0 / b[i]; o0 = div_by_cached_guarded(x, b[i], o1); break;
+        case PB_MATH_BOX_MULLER_F32: box_muller_f32((uint32_t)x, (uint32_t)b[i], o0, o1); break;
+    }
+    out[2 * i] = o0;
+    out[2 * i + 1] = o1;
+}
+cudaError_t launch_debug_math(int op, long long n, const double* a, const double* b, double* out, cudaStream_t s) {
+    debug_math_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(op, n, a, b, out);
+    return cudaGetLastError();
+}

@@ -1353,6 +1353,28 @@ int32_t pb_debug_normals(pb_engine* e, uint64_t seed, uint64_t rng_call, int64_t
     return PB_OK;
 }
 
+int32_t pb_debug_math(pb_engine* e, int32_t op, int64_t n, const double* a, const double* b, double* out) {
+    if (!e || n < 0 || (n && (!a || !out))) return fail(PB_ERR_INVALID, "NULL argument");
+    if (op < PB_MATH_COS_NP || op > PB_MATH_BOX_MULLER_F32) return fail(PB_ERR_INVALID, "unknown math op %d", op);
+    const bool binary = op >= PB_MATH_DIV_BY_CACHED;
+    if (n && binary && !b) return fail(PB_ERR_INVALID, "math op %d needs a second operand", op);
+    CK(cudaSetDevice(e->device));
+    if (n == 0) return PB_OK;
+    double *d_a = nullptr, *d_b = nullptr, *d_out = nullptr;
+    CK(cudaMalloc(&d_a, n * 8));
+    CK(cudaMalloc(&d_out, n * 16));
+    if (binary) CK(cudaMalloc(&d_b, n * 8));
+    CK(cudaMemcpyAsync(d_a, a, n * 8, cudaMemcpyHostToDevice, e->stream));
+    if (binary) CK(cudaMemcpyAsync(d_b, b, n * 8, cudaMemcpyHostToDevice, e->stream));
+    CK(launch_debug_math(op, n, d_a, d_b, d_out, e->stream));
+    CK(cudaMemcpyAsync(out, d_out, n * 16, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    cudaFree(d_a);
+    cudaFree(d_b);
+    cudaFree(d_out);
+    return PB_OK;
+}
+
 
 // ------------------------------------------------------------------------------------------------
 // mode D: X-slab domain decomposition + particle migration (SURVEY.md 8e).  The exchange itself is an

@@ -389,3 +389,15 @@ class Engine:
         out = np.empty((pid.size, 2), dtype=np.float64)
         check(self._lib.pb_debug_normals(self._h, int(seed), int(rng_call), int(it), pid.size, ptr(pid), ptr(out)))
         return out
+
+    # pb_math_op (include/parcels_b200.h)
+    MATH_OPS = {"cos_np": 0, "sin_lat": 1, "sincos_lon": 2, "div_by_cached": 3, "div_by_cached_guarded": 4, "box_muller_f32": 5}
+
+    def debug_math(self, op, a, b=None):
+        """The kernels' math primitive `op` evaluated on the device: (n, 2) float64 (see pb_debug_math)."""
+        a = np.ascontiguousarray(a, dtype=np.float64).ravel()
+        if b is not None:
+            b = np.ascontiguousarray(np.broadcast_to(np.asarray(b, dtype=np.float64), a.shape))
+        out = np.empty((a.size, 2), dtype=np.float64)
+        check(self._lib.pb_debug_math(self._h, self.MATH_OPS[op], a.size, ptr(a), ptr(b), ptr(out)))
+        return out
