@@ -146,7 +146,11 @@ int32_t pb_field_clear(pb_engine* e, int32_t slot);
  * for the next advect calls (stream-ordered after the pending loads).  pb_advect stops a particle whose next
  * step would sample outside the resident levels (pb_report.n_wait_window): slide the window and call
  * pb_advect again with resume = 1.  A step that straddles a time level samples 3 levels, so window_levels = 3 is
- * the general minimum (2 suffices only when no step straddles a level). */
+ * the general minimum (2 suffices only when no step straddles a level).  pb_advect_rk45 and pb_advect_diffusion
+ * wait the same way (RK45: the span [t, t + dt] of the particle's clamped dt; M1 / EM: its time t) and are resumed the
+ * same way; a resumed launch (resume = 1 without kernels_only) continues every particle's loop-iteration count, so the
+ * result -- the Wiener increments of M1 / EM included -- is the resident one bit for bit.  pb_sample_velocity returns
+ * PB_ERR_INVALID when a finite sample time inside the time axis lies outside the resident levels. */
 int32_t pb_field_window_create(pb_engine* e, int32_t slot, int32_t data_is_f64, int64_t T_total, int64_t Z, int64_t Y,
                                int64_t X, int32_t window_levels);
 int32_t pb_field_window_load(pb_engine* e, int32_t slot, int64_t level, const void* host_level_data);
@@ -278,8 +282,11 @@ int32_t pb_advect_host(pb_engine* e, const pb_advect_args* args, int64_t n, cons
  * reference leaves it, including its batch-level clamp of the particles that left the loop early (kernel.py:199-203).
  * pb_report: particle_steps = accepted steps, cache_refills = field evaluations (6 per attempt), n_error = particles
  * whose dt is 0 before endtime (state 50; the reference's loop never terminates on those).
- * Fully resident fields: XLinear_Velocity / XFreeslip / XPartialslip on rectilinear A-grids, CGrid_Velocity on rectilinear and
- * curvilinear C-grids. */
+ * XLinear_Velocity / XFreeslip / XPartialslip on rectilinear A-grids, CGrid_Velocity on rectilinear and curvilinear C-grids,
+ * resident or time-windowed (pb_field_window_create): a particle whose next iteration's span [t, t + dt] is not resident stops
+ * with its state, dt and next_dt unchanged (pb_report.n_wait_window); after pb_field_window_set, call again with resume = 1:
+ * the engine keeps every particle's iteration count between the launches, and clamps the dt of the particles that left the
+ * loop early (above) only after the launch that leaves nobody waiting. */
 typedef struct pb_rk45_args {
     double dt;      /* nominal dt of ParticleSet.execute: only its sign is used (compute_time_direction) */
     double endtime;
@@ -305,7 +312,11 @@ int32_t pb_advect_rk45(pb_engine* e, const pb_rk45_args* args, double* dt_inout,
  * the reference adds to the float32 positions (weak scalar: positions stay float32); deg2m_sq = pow(grid.deg2m, 2).
  * The Wiener increments come from the engine's Philox4x32-10 stream keyed like pb_advect's DiffusionUniformKh (the
  * reference draws from NumPy's global MT19937: statistical parity, bit parity of the deterministic part).
- * Same loop semantics, max_iters replay contract and pb_report as pb_advect.  Resident rectilinear A-grid fields. */
+ * Same loop semantics, max_iters replay contract and pb_report as pb_advect.  Rectilinear grids, resident or time-windowed
+ * U, V: a particle whose time t is not inside the resident levels stops (pb_report.n_wait_window); after
+ * pb_field_window_set, call again with resume = 1 -- the engine keeps every particle's iteration count between the
+ * launches, so the Wiener increments, first_error_iter and max_iters are those of one resident launch.
+ * pb_advect_diffusion_async: the same launch without waiting (pb_last_report collects the report, like pb_advect_async). */
 enum pb_advdiff_scheme { PB_ADVDIFF_M1 = 0, PB_ADVDIFF_EM = 1 };
 typedef struct pb_advdiff_args {
     int32_t scheme;             /* enum pb_advdiff_scheme */
@@ -325,13 +336,15 @@ typedef struct pb_advdiff_args {
     int32_t reserved;
 } pb_advdiff_args;
 int32_t pb_advect_diffusion(pb_engine* e, const pb_advdiff_args* args, pb_report* rep);
+int32_t pb_advect_diffusion_async(pb_engine* e, const pb_advdiff_args* args);
 
 /* VectorField.eval at n arbitrary sample points (fieldset.UV[t, z, y, x] / fieldset.UVW[...],
  * _core/field.py:250-304): time + grid search, interpolation, unit conversion, error states
  * (state_out starts at Evaluate and is raised like particles.state), ei_out = ravel_index of the cell.
  * positions_are_f32 = 1 evaluates with float32 positions (a particle's own arrays), 0 with float64
  * (an RK stage position) -- the reference's arithmetic promotes on that dtype.  ei_hint (may be NULL)
- * seeds the curvilinear search like particles.ei does; no_hint = 1 skips the hint test. */
+ * seeds the curvilinear search like particles.ei does; no_hint = 1 skips the hint test.  Time-windowed U, V, W: every
+ * finite sample time inside the time axis must lie within the resident levels, else PB_ERR_INVALID. */
 int32_t pb_sample_velocity(pb_engine* e, int64_t n, const double* t, const double* z, const double* y, const double* x,
                            int32_t positions_are_f32, int32_t three_d, const int32_t* ei_hint, int32_t no_hint,
                            double* u, double* v, double* w, int32_t* ei_out, int32_t* state_out);

@@ -145,6 +145,7 @@ SYMBOLS = {
     "pb_advect_host": (C.c_int32, [_P, C.POINTER(AdvectArgs), C.c_int64, C.POINTER(ParticleArrays), C.c_int32, C.c_int32, C.POINTER(Report)]),
     "pb_advect_rk45": (C.c_int32, [_P, _P, _P, _P, _P]),
     "pb_advect_diffusion": (C.c_int32, [_P, C.POINTER(AdvDiffArgs), C.POINTER(Report)]),
+    "pb_advect_diffusion_async": (C.c_int32, [_P, C.POINTER(AdvDiffArgs)]),
     "pb_last_report": (C.c_int32, [_P, C.POINTER(Report)]),
     "pb_sample_velocity": (C.c_int32, [_P, C.c_int64, _P, _P, _P, _P, C.c_int32, C.c_int32, _P, C.c_int32, _P, _P, _P, _P, _P]),
     "pb_sample_scalar": (C.c_int32, [_P, C.c_int32, C.c_int32, C.c_int64, _P, _P, _P, _P, C.c_int32, _P, _P, _P, _P, _P]),

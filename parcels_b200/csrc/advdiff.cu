@@ -28,6 +28,7 @@ struct AdvDiffParams {
     double two_dres;    // 2 * fieldset.dres (Python float arithmetic)
     double deg2m;       // Kh_zonal.grid.deg2m
     double deg2m_sq;    // pow(deg2m, 2) as Python computes it
+    int* iters;         // time-windowed fields: each lane's iteration count, kept across the resumed launches of one call (else NULL)
 };
 
 // NumPy-typed scalar helpers on tagged values: Python scalars are weak (cast to the array dtype first)
@@ -56,7 +57,7 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, 2) advdiff_kernel(const AdvD
     unsigned long long my_steps = 0, my_refills = 0;
     int final_state = 0;
     long long my_iters = 0;
-    bool errored = false, deleted = false, oot = false;
+    bool errored = false, deleted = false, oot = false, wait_window = false;
     long long err_iter = LLONG_MAX;
 
     if (i < p.P.n) {
@@ -88,12 +89,22 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, 2) advdiff_kernel(const AdvD
             return val;
         };
 
-        long long it = 0;
+        // a resumed launch of the same Kernel.execute call (time-slab streaming) continues the lane's iteration count: the
+        // Wiener increments (keyed by it), the first-iteration batch rule and max_iters are those of the resident run
+        long long it = (q.iters && p.resume && !p.kernels_only) ? (long long)q.iters[i] : 0;
         for (;; ++it) {
             if (p.max_iters >= 0 && it >= p.max_iters) break;
             const double tte = sign * (p.endtime - t);                                    // kernel.py:191
             if (!((state == PB_SUCCESS || state == PB_EVALUATE) && tte >= 0)) break;      // :193-195
             const double dtp = (sign == 1) ? fmax(fmin(p.dt, tte), 0.0) : fmin(fmax(p.dt, -tte), 0.0);  // :199-203
+            // every sample of M1 / EM is taken at the particle's own time (_advectiondiffusion.py:40-60,87-110): t must lie
+            // within the resident time levels; outside the field's whole time interval is OutsideTimeInterval, not a wait
+            if (p.f.windowed && !(t >= p.f.win_t0 && t <= p.f.win_t1) && t >= 0 && t <= p.g.time_len) {
+                wait_window = true;
+                atomicMin(&p.rep->wait_t_min_bits, (unsigned long long)__double_as_longlong(t));
+                atomicMax(&p.rep->wait_t_max_bits, (unsigned long long)__double_as_longlong(t));
+                break;
+            }
             my_steps++;
             if constexpr (std::is_same<A, float>::value) {
                 // float32 grids: every sample of this kernel is taken at the particle's own time with float32 positions; in the
@@ -170,11 +181,12 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, 2) advdiff_kernel(const AdvD
         p.P.t[i] = t;
         p.P.state[i] = state;
         p.P.ei[i] = ek.ei;
+        if (q.iters) q.iters[i] = (int)it;
     }
 
     const unsigned full = 0xffffffffu;
     unsigned long long s_steps = my_steps, s_ref = my_refills;
-    unsigned n_err = errored, n_del = deleted, n_oot = oot;
+    unsigned n_err = errored, n_del = deleted, n_oot = oot, n_ww = wait_window;
     // with the delete handler an out-of-interval sample is not an error of the lane, but the host still needs the iteration
     // it happened in (the reference deletes the WHOLE evaluated view of that iteration, field.py:31-44)
     long long mx_it = my_iters, mn_err = (oot && deleted) ? my_iters - 1 : err_iter;
@@ -186,6 +198,7 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, 2) advdiff_kernel(const AdvD
         n_err += __shfl_xor_sync(full, n_err, o);
         n_del += __shfl_xor_sync(full, n_del, o);
         n_oot += __shfl_xor_sync(full, n_oot, o);
+        n_ww += __shfl_xor_sync(full, n_ww, o);
         mx_it = max(mx_it, __shfl_xor_sync(full, mx_it, o));
         mn_err = min(mn_err, __shfl_xor_sync(full, mn_err, o));
         mx_state = max(mx_state, __shfl_xor_sync(full, mx_state, o));
@@ -196,6 +209,7 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, 2) advdiff_kernel(const AdvD
         if (n_err) atomicAdd(&p.rep->n_error, (unsigned long long)n_err);
         if (n_del) atomicAdd(&p.rep->n_deleted, (unsigned long long)n_del);
         if (n_oot) atomicAdd(&p.rep->n_out_of_time, (unsigned long long)n_oot);
+        if (n_ww) atomicAdd(&p.rep->n_wait_window, (unsigned long long)n_ww);
         if (mx_it) atomicMax(&p.rep->max_iters_done, mx_it);
         if (mn_err != LLONG_MAX) atomicMin(&p.rep->first_error_iter, mn_err);
         if (mx_state) atomicMax(&p.rep->max_state, mx_state);
@@ -231,9 +245,10 @@ static cudaError_t launch_a(const AdvDiffParams& q, bool d64, bool k64, bool ht,
 
 // scheme 0 = M1, 1 = EM.  uv_/kh_: dtype and time dimension of U,V and of the two Kh fields.
 cudaError_t launch_advdiff(const AdvectParams& p, const FieldDev& fkz, const FieldDev& fkm, int em, double dres, double deg2m_sq,
-                           bool coord_f64, bool uv_f64, bool kh_f64, bool uv_time, bool kh_time, bool cgrid, cudaStream_t s) {
+                           bool coord_f64, bool uv_f64, bool kh_f64, bool uv_time, bool kh_time, bool cgrid, int* iters, cudaStream_t s) {
     AdvDiffParams q{};
     q.base = p;
+    q.iters = iters;
     q.fkz = fkz; q.fkm = fkm;
     q.em = em;
     q.spherical = p.g.spherical;

@@ -315,6 +315,7 @@ struct pb_engine {
     // output path: block counts / offsets of the ordered selection, selected indices, compacted columns
     DevBuf sblock, soffs, sidx, sout;
     DevBuf samp_d, samp_i;  // scratch of pb_sample_velocity / pb_sample_scalar (grown on demand, reused across calls)
+    DevBuf ad_iters;        // time-slab streaming: pb_advect_diffusion's per-particle iteration counts across resumed launches
     long long* h_sel_total = nullptr;  // pinned
     long long n_selected = -1;
     // in-kernel migration over peer memory: own inbox allocation, every rank's inbox as mapped here, the slot of this round
@@ -417,7 +418,7 @@ void pb_engine_destroy(pb_engine* e) {
     e->il.release();
     for (DevBuf* b : {&e->hqbox, &e->hbucket, &e->cellproj, &e->hkeys, &e->hstarts, &e->hcounts, &e->hfaces, &e->lon, &e->lat, &e->depth, &e->time, &e->px, &e->py, &e->pz,
                       &e->pdx, &e->pdy, &e->pdz, &e->pt, &e->pstate, &e->pei, &e->ppid, &e->snap, &e->sblock, &e->soffs, &e->sidx, &e->sout,
-                      &e->samp_d, &e->samp_i})
+                      &e->samp_d, &e->samp_i, &e->ad_iters})
         b->release();
     for (int r = 0; r < PB_MIG_MAX_RANKS; ++r)
         if (e->mig_ipc_opened[r]) cudaIpcCloseMemHandle(e->mig_peer[r]);
@@ -853,6 +854,19 @@ int32_t pb_sample_velocity(pb_engine* e, int64_t n, const double* t, const doubl
     int32_t rc = check_fields(e, nc);
     if (rc) return rc;
     if (n == 0) return PB_OK;
+    if (e->ring && !e->time_host.empty()) {
+        // time-windowed U, V, W: a finite sample time inside the time axis needs its levels resident (outside the axis is
+        // OutsideTimeInterval and reads nothing); otherwise its ring slot may hold another level
+        const double ax0 = e->time_host.front(), ax1 = e->time_host.back();
+        const double w0 = e->win_n > 0 ? e->time_host[e->win_first] : 0.0;
+        const double w1 = e->win_n > 0 ? e->time_host[e->win_first + e->win_n - 1] : -1.0;
+        double lo = HUGE_VAL, hi = -HUGE_VAL;
+        for (int64_t k = 0; k < n; ++k)
+            if (t[k] >= ax0 && t[k] <= ax1) { lo = t[k] < lo ? t[k] : lo; hi = t[k] > hi ? t[k] : hi; }
+        if (lo <= hi && !(lo >= w0 && hi <= w1))
+            return fail(PB_ERR_INVALID, "sample times [%.17g, %.17g] are not all inside the resident time levels [%.17g, %.17g]: "
+                                        "pb_field_window_set first", lo, hi, w0, w1);
+    }
     CK(cudaSetDevice(e->device));
     if ((rc = e->samp_d.ensure((size_t)n * 7 * sizeof(double)))) return rc;
     if ((rc = e->samp_i.ensure(((size_t)n * 3 + 1) * sizeof(int)))) return rc;
@@ -1202,13 +1216,13 @@ int32_t pb_advect_rk45(pb_engine* e, const pb_rk45_args* a, double* dt_inout, do
     if (rc) return rc;
     const bool cgrid = e->interp == PB_INTERP_CGRID_VELOCITY;
     const bool slip = agrid_alt_mode(e->interp) == 1;
-    if (!(cgrid || ((e->interp == PB_INTERP_XLINEAR_VELOCITY || slip) && !e->g.curvilinear)) || e->ring || e->g.decomposed)
-        return fail(PB_ERR_INVALID, "AdvectionRK45 runs on resident fields with XLinear_Velocity / XFreeslip / XPartialslip (rectilinear A-grid) "
-                                    "or CGrid_Velocity");
+    if (!(cgrid || ((e->interp == PB_INTERP_XLINEAR_VELOCITY || slip) && !e->g.curvilinear)) || e->g.decomposed)
+        return fail(PB_ERR_INVALID, "AdvectionRK45 runs on XLinear_Velocity / XFreeslip / XPartialslip (rectilinear A-grid) "
+                                    "or CGrid_Velocity fields, not under domain decomposition");
     CK(cudaSetDevice(e->device));
     const size_t n = (size_t)e->n;
     DevBuf& buf = e->sout;  // dt, next_dt (f64), iters (i32)
-    if ((rc = buf.ensure(n ? n * 20 : 1))) return rc;
+    if ((rc = buf.ensure(n ? n * 20 : 1))) return rc;  // (kept as it is across resumed launches: the iteration counts live here)
     double* d_dt = (double*)buf.p;
     double* d_ndt = d_dt + n;
     int* d_it = (int*)(d_ndt + n);
@@ -1246,7 +1260,9 @@ int32_t pb_advect_rk45(pb_engine* e, const pb_rk45_args* a, double* dt_inout, do
     e->pending = true;
     if ((rc = pb_last_report(e, rep))) return rc;
     if (n) {
-        if (!a->kernels_only) {  // (in a mixed list the host clamps every particle's dt at the top of each iteration itself)
+        // once, after the last launch of the call: a launch that left lanes waiting for the time window is resumed, and the
+        // counts it left in d_it are continued.  (In a mixed list the host clamps every particle's dt at the top of each iteration.)
+        if (!a->kernels_only && rep->n_wait_window == 0) {
             cudaError_t ce = launch_rk45_finalize(p.P, d_dt, d_it, rep->max_iters_done, a->endtime, a->dt > 0 ? 1 : -1, e->stream);
             if (ce != cudaSuccess) return fail(PB_ERR_CUDA, "rk45_finalize launch failed: %s", cudaGetErrorString(ce));
         }
@@ -1273,16 +1289,17 @@ static int32_t scalar_field_desc(pb_engine* e, int32_t slot, FieldDev& f) {
     return PB_OK;
 }
 
-int32_t pb_advect_diffusion(pb_engine* e, const pb_advdiff_args* a, pb_report* rep) {
+int32_t pb_advect_diffusion_async(pb_engine* e, const pb_advdiff_args* a) {
     PB_RANGE("pb_advect_diffusion");
-    if (!e || !a || !rep) return fail(PB_ERR_INVALID, "NULL argument");
+    if (!e || !a) return fail(PB_ERR_INVALID, "NULL argument");
     if (a->dt == 0.0 || a->dt != a->dt) return fail(PB_ERR_INVALID, "dt must be a non-zero number");
     if (a->scheme != PB_ADVDIFF_M1 && a->scheme != PB_ADVDIFF_EM) return fail(PB_ERR_INVALID, "unknown advection-diffusion scheme %d", a->scheme);
     if (!(a->dres == a->dres) || a->dres == 0.0) return fail(PB_ERR_INVALID, "dres must be a non-zero number");
     int32_t rc = check_fields(e, 2);
     if (rc) return rc;
-    if ((e->interp != PB_INTERP_XLINEAR_VELOCITY && e->interp != PB_INTERP_CGRID_VELOCITY) || e->g.curvilinear || e->ring || e->g.decomposed)
-        return fail(PB_ERR_INVALID, "AdvectionDiffusionM1/EM run on resident rectilinear fields with XLinear_Velocity or CGrid_Velocity");
+    if ((e->interp != PB_INTERP_XLINEAR_VELOCITY && e->interp != PB_INTERP_CGRID_VELOCITY) || e->g.curvilinear || e->g.decomposed)
+        return fail(PB_ERR_INVALID, "AdvectionDiffusionM1/EM run on rectilinear fields with XLinear_Velocity or CGrid_Velocity, "
+                                    "not under domain decomposition");
     if (!e->have_pid) return fail(PB_ERR_STATE, "diffusion needs particle_id (RNG counter)");
     FieldDev fkz, fkm;
     if ((rc = scalar_field_desc(e, a->kh_zonal_slot, fkz))) return rc;
@@ -1300,18 +1317,31 @@ int32_t pb_advect_diffusion(pb_engine* e, const pb_advdiff_args* a, pb_report* r
     p.kernels_only = a->kernels_only; p.resume = a->resume;
     p.batch_levels = a->batch_levels;
     p.rep = e->d_rep;
+    // time-windowed fields: the lanes' iteration counts survive into the resumed launches (resident fields need none)
+    int* iters = nullptr;
+    if (e->ring) {
+        if ((rc = e->ad_iters.ensure(e->n ? (size_t)e->n * sizeof(int) : 1))) return rc;
+        iters = (int*)e->ad_iters.p;
+    }
     zero_report(*e->h_rep);
     CK(cudaMemcpyAsync(e->d_rep, e->h_rep, sizeof(ReportDev), cudaMemcpyHostToDevice, e->stream));
     CK(cudaEventRecord(e->ev0, e->stream));
     if (e->n > 0) {
         cudaError_t ce = launch_advdiff(p, fkz, fkm, a->scheme == PB_ADVDIFF_EM, a->dres, a->deg2m_sq, e->coord_f64 != 0, e->f_f64[0] != 0,
                                         e->f_f64[a->kh_zonal_slot] != 0, e->g.nt > 0, fkz.T > 1, e->interp == PB_INTERP_CGRID_VELOCITY,
-                                        e->stream);
+                                        iters, e->stream);
         if (ce != cudaSuccess) return fail(PB_ERR_CUDA, "advdiff_kernel launch failed: %s", cudaGetErrorString(ce));
     }
     CK(cudaEventRecord(e->ev1, e->stream));
     CK(cudaMemcpyAsync(e->h_rep, e->d_rep, sizeof(ReportDev), cudaMemcpyDeviceToHost, e->stream));
     e->pending = true;
+    return PB_OK;
+}
+
+int32_t pb_advect_diffusion(pb_engine* e, const pb_advdiff_args* a, pb_report* rep) {
+    if (!rep) return fail(PB_ERR_INVALID, "NULL argument");
+    int32_t rc = pb_advect_diffusion_async(e, a);
+    if (rc) return rc;
     return pb_last_report(e, rep);
 }
 

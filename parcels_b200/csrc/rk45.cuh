@@ -7,7 +7,8 @@ struct Rk45Params {
     AdvectParams base;   // grid, field, particles, dt (sign), endtime, max_iters, report
     double* dt;          // per-particle dt (particles.dt, float64)
     double* next_dt;     // per-particle next_dt, widened to float64
-    int* iters;          // loop iterations each particle took part in (for the batch-level clamp, below)
+    int* iters;          // loop iterations each particle took part in (for the batch-level clamp, below); a launch that
+                         // continues the previous one after a time-window wait (resume without kernels_only) starts from it
     int next_dt_f32;     // the Particle's next_dt Variable is float32 (the default dtype): round on assignment
     double tol, min_dt, max_dt;
 };
@@ -21,7 +22,7 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, PB_MINBLOCKS) rk45_kernel(co
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     unsigned long long my_steps = 0, my_evals = 0;
     long long my_iters = 0;
-    bool stalled = false;
+    bool stalled = false, wait_window = false;
     int final_state = 0;
     if (i < p.P.n) {
         // Butcher tableau of _advection.py:96-106, the same Python float expressions
@@ -48,7 +49,9 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, PB_MINBLOCKS) rk45_kernel(co
         }
         const int sign = p.dt > 0 ? 1 : -1;  // compute_time_direction (kernel.py:186)
         bool first_attempt = true;
-        long long it = 0;
+        // a resumed launch of the same Kernel.execute call (time-slab streaming) continues the lane's iteration count, so the
+        // first-iteration batch rules, max_iters and the finalize clamp see the iterations of the whole call
+        long long it = (p.resume && !p.kernels_only) ? (long long)q.iters[i] : 0;
         for (;; ++it) {
             if (p.max_iters >= 0 && it >= p.max_iters) break;
             const double tte = sign * (p.endtime - t);
@@ -57,6 +60,17 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, PB_MINBLOCKS) rk45_kernel(co
             if (dt == 0.0 && tte > 0) {  // the reference never terminates here (t cannot advance): report instead of spinning
                 stalled = true;
                 break;
+            }
+            if (p.f.windowed) {
+                // every attempt of this iteration samples inside [t, t + dt] (a rejected attempt halves dt), so that span must
+                // lie within the resident time levels; outside the field's whole time interval is OutsideTimeInterval, not a wait
+                const double ta = fmin(t, t + dt), tb = fmax(t, t + dt);
+                if (!(ta >= p.f.win_t0 && tb <= p.f.win_t1) && ta >= 0 && tb <= p.g.time_len) {
+                    wait_window = true;  // state, dt and next_dt stay as they are: the resumed launch repeats this iteration
+                    atomicMin(&p.rep->wait_t_min_bits, (unsigned long long)__double_as_longlong(t));
+                    atomicMax(&p.rep->wait_t_max_bits, (unsigned long long)__double_as_longlong(t));
+                    break;
+                }
             }
             my_steps++;
             do {  // kernel.py:206-216: the kernel, then again for as long as it asks to be repeated
@@ -154,7 +168,7 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, PB_MINBLOCKS) rk45_kernel(co
     }
     const unsigned full = 0xffffffffu;
     unsigned long long s_steps = my_steps, s_ev = my_evals;
-    unsigned n_stall = stalled;
+    unsigned n_stall = stalled, n_ww = wait_window;
     long long mx_it = my_iters;
     int mx_state = final_state;
 #pragma unroll
@@ -162,6 +176,7 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, PB_MINBLOCKS) rk45_kernel(co
         s_steps += __shfl_xor_sync(full, s_steps, o);
         s_ev += __shfl_xor_sync(full, s_ev, o);
         n_stall += __shfl_xor_sync(full, n_stall, o);
+        n_ww += __shfl_xor_sync(full, n_ww, o);
         mx_it = max(mx_it, __shfl_xor_sync(full, mx_it, o));
         mx_state = max(mx_state, __shfl_xor_sync(full, mx_state, o));
     }
@@ -169,6 +184,7 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, PB_MINBLOCKS) rk45_kernel(co
         if (s_steps) atomicAdd(&p.rep->particle_steps, s_steps);
         if (s_ev) atomicAdd(&p.rep->cache_refills, s_ev);  // RK45: the number of field evaluations (6 per attempt)
         if (n_stall) atomicAdd(&p.rep->n_error, (unsigned long long)n_stall);
+        if (n_ww) atomicAdd(&p.rep->n_wait_window, (unsigned long long)n_ww);
         if (mx_it) atomicMax(&p.rep->max_iters_done, mx_it);
         if (mx_state) atomicMax(&p.rep->max_state, mx_state);
     }

@@ -268,8 +268,14 @@ class Engine:
         check(self._lib.pb_advect_host(self._h, C.byref(args), n, C.byref(h), int(bool(download)), int(n_chunks), C.byref(rep)))
         return _report_dict(rep)
 
-    def advect_async(self, args: AdvectArgs):
-        check(self._lib.pb_advect_async(self._h, C.byref(args)))
+    def advect_async(self, args):
+        """:meth:`advect` without waiting for the kernel; :meth:`last_report` waits and returns the report."""
+        from ._lib import AdvDiffArgs
+
+        if isinstance(args, AdvDiffArgs):
+            check(self._lib.pb_advect_diffusion_async(self._h, C.byref(args)))
+        else:
+            check(self._lib.pb_advect_async(self._h, C.byref(args)))
 
     def last_report(self) -> dict:
         rep = Report()

@@ -30,6 +30,21 @@ def window_range(time_s, t, sign: int, window: int) -> tuple[int, int]:
     return first, min(window, T - first)
 
 
+def window_span(time_s, lo, hi, sign: int, window: int) -> tuple[int, int] | None:
+    """Time levels [first, first + n) to keep resident so that every sample time in [lo, hi] (inside the time axis) reads
+    resident levels; the window extends in direction ``sign`` beyond the span.  None when the span needs more than ``window``
+    levels."""
+    T = len(time_s)
+    first = int(np.clip(np.searchsorted(time_s, lo, side="right") - 1, 0, max(T - 2, 0)))
+    last = int(np.clip(np.searchsorted(time_s, hi, side="left"), 1, T - 1))
+    if last - first + 1 > window:
+        return None
+    if sign < 0:
+        first = max(0, last - window + 1)
+    first = min(first, max(T - window, 0))
+    return first, min(window, T - first)
+
+
 def _to_seconds(time):
     """time axis -> (float64 seconds since the first level, origin) (reference index_search.py:88)."""
     if time is None:
@@ -220,7 +235,10 @@ class VectorField:
         hint = None
         if particles is not None:
             hint = np.ascontiguousarray(np.asarray(particles.ei)[:, -1])
-        u, v, w, ei, st = host.engine(device).sample_velocity(t, z, y, x, three_d=self.W is not None, positions_are_f32=positions_are_f32,
+        eng = host.engine(device)
+        if host is fs and fs.time_window is not None:
+            fs.cover_window(device, t)  # time-windowed U, V, W: the batch's levels resident (times outside the axis: OutsideTimeInterval)
+        u, v, w, ei, st = eng.sample_velocity(t, z, y, x, three_d=self.W is not None, positions_are_f32=positions_are_f32,
                                                               ei_hint=hint, no_hint=_batch_skips_hint(self.grid, hint))  # fmt: skip
         if particles is not None:
             from .statuscodes import StatusCode
@@ -538,9 +556,28 @@ class FieldSet:
 
     def slide_window(self, device, t, sign):
         """Make the levels a particle at time ``t`` needs resident; returns True if the window moved."""
+        return self._set_window(device, *window_range(self._time_s, t, sign, self.time_window))
+
+    def cover_window(self, device, t, sign=1):
+        """Make the levels of every finite sample time in ``t`` that lies inside the time axis resident (a step-by-step kernel
+        list, a user kernel's ``fieldset.UV[...]``).  Raises RuntimeError when no window of ``time_window`` levels holds them."""
+        t = np.asarray(t, dtype=np.float64)
+        inside = t[(t >= self._time_s[0]) & (t <= self._time_s[-1])]  # (NaN fails both tests)
+        if inside.size == 0:
+            return
+        lo, hi = float(inside.min()), float(inside.max())
+        w = self._win[device]
+        if w["n"] and self._time_s[w["first"]] <= lo and hi <= self._time_s[w["first"] + w["n"] - 1]:
+            return
+        span = window_span(self._time_s, lo, hi, sign, self.time_window)
+        if span is None:
+            raise RuntimeError(f"sample times {lo} .. {hi} span more than the {self.time_window} resident time levels of this "
+                               "FieldSet: widen time_window")  # fmt: skip
+        self._set_window(device, *span)
+
+    def _set_window(self, device, first, n):
         eng = self._engines[device]
         w = self._win[device]
-        first, n = window_range(self._time_s, t, sign, self.time_window)
         moved = (first, n) != (w["first"], w["n"])
         for lv in range(first, first + n):
             if lv not in w["resident"]:

@@ -254,9 +254,10 @@ class KernelPlan:
         if "DiffusionUniformKh" in tokens and any(n in K.ADVDIFF for n in tokens if n):
             raise NotImplementedError("AdvectionDiffusionM1/EM already diffuse: combining them with DiffusionUniformKh is not supported")
         self.stepwise = not (len(names) == 1 and names[0] in K.SCHEMES)
-        if fieldset.time_window is not None and (self.stepwise or not self.delete_on_error):
-            raise NotImplementedError("time-windowed FieldSets need a list of built-in kernels ending with the DeleteParticle token: "
-                                      "an error cannot be replayed step-exactly once the window has moved on")  # fmt: skip
+        if fieldset.time_window is not None and not self.delete_on_error:
+            # without the DeleteParticle token an error must stop the whole set at the end of its iteration; the fused kernel
+            # could only replay that iteration from the start of the interval, whose time levels the window has left behind
+            self.stepwise = True
         if self.stepwise:
             # the list mixes built-ins with user Python kernels: the loop control runs on the host step by step
             # (stepwise.py), every built-in kernel still runs on the device
@@ -311,8 +312,8 @@ def _setup_rk45(self, names, fieldset, pclass):
     if pclass is None or "next_dt" not in [v.name for v in pclass.variables]:
         raise ValueError('ParticleClass requires a "next_dt" for AdvectionRK45 Kernel.')
     if not ((fieldset.interp_method in ("linear", "freeslip", "partialslip") and not fieldset.grid.curvilinear)
-            or fieldset.interp_method == "cgrid_velocity") or fieldset.time_window is not None:  # fmt: skip
-        raise NotImplementedError("AdvectionRK45 is implemented for resident fields with XLinear_Velocity, XFreeslip or XPartialslip "
+            or fieldset.interp_method == "cgrid_velocity"):  # fmt: skip
+        raise NotImplementedError("AdvectionRK45 is implemented for XLinear_Velocity, XFreeslip or XPartialslip "
                                   "(rectilinear A-grids) or CGrid_Velocity (rectilinear and curvilinear C-grids)")
     ctx = fieldset.context
     if "RK45_tol" not in ctx:
@@ -363,8 +364,8 @@ def _advdiff_params(fieldset, name):
     if kz._slot is None or km._slot is None or kz.interp_method != "linear" or km.interp_method != "linear":
         raise NotImplementedError(f"{name}: Kh_zonal / Kh_meridional must be XLinear scalar fields on the FieldSet's grid "
                                   "(FieldSet.add_field(name, data)); constant fields have no gradient -- use DiffusionUniformKh")  # fmt: skip
-    if fieldset.grid.curvilinear or fieldset.interp_method not in ("linear", "cgrid_velocity") or fieldset.time_window is not None:
-        raise NotImplementedError(f"{name} is implemented for resident rectilinear fields (XLinear_Velocity or CGrid_Velocity)")
+    if fieldset.grid.curvilinear or fieldset.interp_method not in ("linear", "cgrid_velocity"):
+        raise NotImplementedError(f"{name} is implemented for rectilinear fields (XLinear_Velocity or CGrid_Velocity)")
     if kz.data.dtype != km.data.dtype or (kz.data.shape[0] > 1) != (km.data.shape[0] > 1):
         raise NotImplementedError("Kh_zonal and Kh_meridional must share dtype and time dimension")
     if "dres" not in fieldset.context:
@@ -636,6 +637,8 @@ class ParticleSet:
         if len(self) == 0:
             return
         eng = self.fieldset.engine(self.device)
+        if self.fieldset.time_window is not None:  # (only the cells are used, but a windowed engine samples resident levels only)
+            self.fieldset.cover_window(self.device, np.zeros(1))
         *_, ei, _ = eng.sample_velocity(np.zeros(len(self)), d["z"], d["y"], d["x"], three_d=False, positions_are_f32=True,
                                         ei_hint=None, no_hint=True)  # fmt: skip
         d["ei"][:, 0] = ei
@@ -737,8 +740,29 @@ class ParticleSet:
         if lazy and not pipelined and (can_raise or self.fieldset.time_interval is not None):
             eng.snapshot()
         rewind = eng.restore if (lazy or pipelined) else (lambda: eng.upload_particles(d, ei_last))
-        if self.fieldset.time_window is not None:
-            rep = self._advect_windowed(eng, plan, d, dt, endtime, args)
+        windowed = self.fieldset.time_window is not None
+
+        def advance(max_iters=-1):
+            """One Kernel.execute on the device particles (up to ``max_iters`` loop iterations)."""
+            if not windowed:
+                return eng.advect(args(max_iters=max_iters))
+
+            def launch(resume):
+                if resume and plan.diffusion:
+                    # the Wiener increments of DiffusionUniformKh are keyed by (particle, iteration OF THE LAUNCH, call): a resumed
+                    # advect_kernel restarts its iteration count, so it gets its own call index -- otherwise the same increments
+                    # would be drawn again.  (pb_advect_diffusion continues each particle's count: its stream needs no new index.)
+                    self._rng_call += 1
+                a = args(max_iters=max_iters)
+                a.resume = int(resume)
+                eng.advect_async(a)
+
+            return self._advect_windowed(eng, d, dt, endtime, launch)
+
+        # pb_advect_diffusion counts the iterations of a windowed call across its launches: its replay is exact as well
+        replayable = not windowed or plan.advdiff is not None
+        if windowed:
+            rep = advance()
         elif pipelined:
             # the result comes back with the same call when somebody is going to read it on the host anyway
             downloaded = not lazy or self.eager_host
@@ -755,21 +779,21 @@ class ParticleSet:
                 if filler is not None:
                     filler.join()
         else:
-            rep = eng.advect(args())
-        if rep["n_error"] > 0 and self.fieldset.time_window is None:
+            rep = advance()
+        if rep["n_error"] > 0 and replayable:
             # The reference stops the whole set at the END of the first loop iteration in which any
             # particle is in an error state (kernel.py:239-245).  Replay from the start-of-interval copy up to
             # and including that iteration so every particle is left exactly where the reference leaves it.
             k = rep["first_error_iter"]
             rewind()
             downloaded = False
-            rep = eng.advect(args(max_iters=k + 1))
+            rep = advance(k + 1)
             if rep["n_out_of_time"] > 0:
                 # an out-of-interval sample flags the WHOLE evaluated view (index_search.py:85-86, field.py:31-44)
                 rewind()
-                eng.advect(args(max_iters=k))
+                advance(k)
                 eng.flag_view_outside_time(dt, endtime)
-        elif plan.delete_on_error and rep["n_out_of_time"] > 0 and self.fieldset.time_window is None:
+        elif plan.delete_on_error and rep["n_out_of_time"] > 0 and replayable:
             # Same whole-view rule under the DeleteParticle handler: every particle evaluated in the first iteration in which ANY
             # particle sampled outside the time interval is flagged, hence deleted (field.py:31-44 then the handler) -- replay up
             # to that iteration, then delete the view.  (The lanes deleted their own out-of-interval particle; the others ran on.)
@@ -777,7 +801,7 @@ class ParticleSet:
             rewind()
             downloaded = False
             first = rep
-            rep = eng.advect(args(max_iters=k))
+            rep = advance(k)
             eng.delete_view_outside_time(dt, endtime)
             rep["n_deleted"] += 1
             rep["max_state"] = max(rep["max_state"], int(StatusCode.Delete))
@@ -856,8 +880,16 @@ class ParticleSet:
             sign = 1 if dt > 0 else -1
             hint_all_zero = _hint_all_zero(ei_last, lambda s_: sign * (endtime - d["t"][s_]) >= 0, self.fieldset.grid.xdim)
         two_levels = _batch_levels(self.fieldset, d, lambda: (1 if dt > 0 else -1) * (endtime - d["t"]) >= 0)
-        rep = eng.advect_rk45(dt, endtime, tol, min_dt, max_dt, dt_arr, ndt_arr, next_dt_is_f32=d["next_dt"].dtype == np.float32,
-                              delete_on_error=plan.delete_on_error, hint_all_zero=hint_all_zero, batch_levels=two_levels)  # fmt: skip
+
+        def launch(resume):  # (a resumed launch continues every particle's dt, next_dt and iteration count)
+            return eng.advect_rk45(dt, endtime, tol, min_dt, max_dt, dt_arr, ndt_arr, next_dt_is_f32=d["next_dt"].dtype == np.float32,
+                                   delete_on_error=plan.delete_on_error, hint_all_zero=hint_all_zero, batch_levels=two_levels,
+                                   resume=resume)  # fmt: skip
+
+        if self.fieldset.time_window is not None:
+            rep = self._advect_windowed(eng, d, dt, endtime, launch, synchronous=True)
+        else:
+            rep = launch(False)
         self.last_report = rep
         eng.download_particles(d, ei_last)
         _store_ei(d, ei_last)
@@ -873,9 +905,12 @@ class ParticleSet:
             if len(dele) > 0:
                 self.remove_indices(dele)
 
-    def _advect_windowed(self, eng, plan, d, dt, endtime, args):
-        """Time-slab streaming: advance until every particle reached ``endtime``, sliding the resident time
-        levels as the particles' clock crosses them; the next level is copied while the kernel runs."""
+    def _advect_windowed(self, eng, d, dt, endtime, launch, *, synchronous=False):
+        """Time-slab streaming: advance until every particle reached ``endtime``, sliding the resident time levels as the
+        particles' clock crosses them.  ``launch(resume)`` runs one launch of the call on the device particles -- pb_advect,
+        pb_advect_diffusion or pb_advect_rk45 -- with ``resume`` from the second launch on.  An asynchronous launch returns
+        None and the next level is copied while its kernel runs.  A ``synchronous`` one (pb_advect_rk45: it brings dt / next_dt
+        back) returns its report; the next level is copied before it, under the kernel only when the level data is pinned."""
         fs = self.fieldset
         sign = 1 if dt > 0 else -1
         todo = sign * (endtime - d["t"]) >= 0
@@ -884,22 +919,22 @@ class ParticleSet:
         total = None
         first = True
         while True:
-            if not first and plan.diffusion:
-                # the Wiener increments are keyed by (particle, iteration OF THE LAUNCH, call): a resumed launch restarts its
-                # iteration count, so it gets its own call index -- otherwise the same increments would be drawn again
-                self._rng_call += 1
-            a = args()
-            a.resume = 0 if first else 1
-            eng.advect_async(a)
-            fs.prefetch_next(self.device, sign)  # H2D of the next level overlaps the kernel
-            rep = eng.last_report()
+            if synchronous:
+                fs.prefetch_next(self.device, sign)
+            rep = launch(not first)
+            if not synchronous:
+                fs.prefetch_next(self.device, sign)  # H2D of the next level overlaps the kernel
+                rep = eng.last_report()
             if total is None:
                 total = dict(rep)
             else:
-                for k in ("particle_steps", "cache_refills", "kernel_ms"):
+                for k in ("particle_steps", "cache_refills", "kernel_ms", "n_error", "n_deleted", "n_out_of_time"):
                     total[k] += rep[k]
-                for k in ("n_error", "n_deleted", "max_state", "n_out_of_time", "first_error_iter", "n_wait_window"):
-                    total[k] = rep[k]
+                for k in ("max_state", "max_iters_done"):
+                    total[k] = max(total[k], rep[k])
+                if rep["first_error_iter"] >= 0 and not 0 <= total["first_error_iter"] <= rep["first_error_iter"]:
+                    total["first_error_iter"] = rep["first_error_iter"]
+                total["n_wait_window"] = rep["n_wait_window"]
             first = False
             if rep["n_wait_window"] == 0:
                 return total

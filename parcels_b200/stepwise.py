@@ -5,8 +5,12 @@ handler, periodic-boundary or ageing kernels; reference ``_core/kernel.py:174-24
 The loop control of one ``Kernel.execute`` call runs here, step by step, exactly as in the reference; every
 BUILT-IN kernel of the list is still executed on the device (``pb_advect(kernels_only=1)``: one iteration's kernel
 functions on the evaluated particles), user functions are called on the host with a ``ParticleSetView``.  The
-price is one host<->device round trip of the particle SoA per time step; lists made of built-ins only never come
-here (they run the whole loop in one kernel launch).
+price is one host<->device round trip of the particle SoA per time step; lists made of built-ins only come here only
+on a time-windowed FieldSet without the DeleteParticle token (elsewhere they run the whole loop in one kernel launch).
+
+On a time-windowed FieldSet every device launch of an iteration first makes the levels of the evaluated particles'
+steps [t, t + dt] resident (``FieldSet.cover_window``); user kernels' ``fieldset.UV[...]`` do the same for their own
+sample times.  An iteration whose particles are spread over more time levels than the window holds raises.
 """
 
 from __future__ import annotations
@@ -37,6 +41,8 @@ def kernel_execute_stepwise(pset, plan, endtime: float, dt: float):
         d["dt"][:] = np.maximum(np.minimum(d["dt"], tte), 0) if sign == 1 else np.minimum(np.maximum(d["dt"], -tte), 0)
         steps += int(np.count_nonzero(evaluate))
         for item in plan.items:
+            if item[0] != "python" and fs.time_window is not None:
+                _cover_steps(pset, evaluate, sign)
             if item[0] in ("device", "advdiff"):
                 _device_kernels(pset, eng, item, dt, endtime)
             elif item[0] == "rk45":
@@ -76,6 +82,25 @@ def kernel_execute_stepwise(pset, plan, endtime: float, dt: float):
     pset.last_report = dict(particle_steps=steps, mode="stepwise")
 
 
+def _cover_steps(pset, evaluate, sign):
+    """Time-windowed U, V, W: make the levels of this iteration's steps [t, t + dt] (dt after the endtime clamp) of the
+    evaluated particles resident -- the part of them inside the time axis (outside it is OutsideTimeInterval)."""
+    fs = pset.fieldset
+    d = pset._data
+    ta = d["t"][evaluate]
+    tb = ta + d["dt"][evaluate]
+    lo, hi = np.minimum(ta, tb), np.maximum(ta, tb)
+    t0, t1 = float(fs._time_s[0]), float(fs._time_s[-1])
+    meets = (hi >= t0) & (lo <= t1)
+    if np.any(meets):
+        fs.cover_window(pset.device, np.clip([lo[meets].min(), hi[meets].max()], t0, t1), sign)
+
+
+def _no_wait(rep):
+    if rep["n_wait_window"] > 0:  # (the iteration's levels were made resident before the launch)
+        raise RuntimeError(f"{rep['n_wait_window']} particles found their time levels not resident: widen time_window")
+
+
 def _device_kernels(pset, eng, item, dt, endtime):
     """One iteration of the built-in kernels ``item`` on the device: the kernel applies the reference's own
     evaluate mask (state in {Success, Evaluate} and time-to-endtime >= 0) and dt clamp, accumulates dx/dy/dz and
@@ -108,6 +133,7 @@ def _device_kernels(pset, eng, item, dt, endtime):
                              kh_deg2m=plan.kh_deg2m, seed=pset.seed, rng_call=pset._rng_call, hint_all_zero=hint_all_zero,
                              resume=True, kernels_only=True, batch_levels=two_levels)  # fmt: skip
     rep = eng.advect(args)
+    _no_wait(rep)
     eng.download_particles(d, ei_last)
     d["ei"][:, -1] = ei_last
     if rep["n_out_of_time"] > 0:  # the reference flags the whole evaluated view (index_search.py:85-86, field.py:31-44)
@@ -145,6 +171,7 @@ def _device_rk45(pset, eng, params, dt, endtime):
     )
     rep = eng.advect_rk45(dt, endtime, tol, min_dt, max_dt, dt_arr, ndt_arr, next_dt_is_f32=d["next_dt"].dtype == np.float32,
                           kernels_only=True, resume=True, hint_all_zero=hint_all_zero, batch_levels=two_levels)  # fmt: skip
+    _no_wait(rep)
     eng.download_particles(d, ei_last)
     d["ei"][:, -1] = ei_last
     d["dt"][:] = dt_arr

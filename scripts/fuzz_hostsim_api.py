@@ -7,7 +7,8 @@ bit-exact, so any difference is the bookkeeping's.
        loop control on the host), in-place edits through the
        arrays the attributes return, `pset[i].x = ...` / `pset[mask].y = ...` views, `pset.z = ...`, remove_indices, add(),
        plain reads (len, attribute access), a second ParticleSet on the same FieldSet executing in between.
-Run:  PB_LIB=oracle/_build/hostsim/libparcels_b200_hostsim.so PB_HOSTSIM_TEST=1 python scripts/fuzz_hostsim_api.py [n] [seed]"""
+Run:  PB_LIB=oracle/_build/hostsim/libparcels_b200_hostsim.so PB_HOSTSIM_TEST=1 python scripts/fuzz_hostsim_api.py [n] [seed]
+      [--windowed-lists]: on time-windowed fieldsets also run the lists without the handler and the lists with user kernels"""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
@@ -23,6 +24,7 @@ warnings.simplefilter("ignore")
 ERR_NAME = {60: "FieldOutOfBoundError", 61: "FieldOutOfBoundSurfaceError", 70: "OutsideTimeInterval", 51: "FieldInterpolationError",
             52: "GridSearchingError", 50: "GeneralError"}
 VERBOSE = os.environ.get("FUZZ_VERBOSE") == "1"
+WINDOWED_LISTS = "--windowed-lists" in sys.argv
 KEYS = ("particle_id", "state", "t", "ei", "x", "y", "z", "dx", "dy", "dz", "dt")
 
 
@@ -69,7 +71,7 @@ def one_case(rng):
         spec["release"] = ("const", 0.0)
     c = cases.build(spec)
     # time-slab streaming in a quarter of the cases with a time axis: 2 or 3 of the levels resident, slid as the set's clock advances
-    # across the calls of the sequence (lists need the DeleteParticle handler there: the other executes are skipped)
+    # across the calls of the sequence (without --windowed-lists only the lists with the DeleteParticle handler run there)
     window = int(rng.choice([2, 3])) if (nt == 4 and rng.random() < 0.4) else None
     if window:
         fs = pb.FieldSet.from_arrays(lon=c["lon"], lat=c["lat"], depth=c["depth"], time=c["times"], U=c["U"], V=c["V"], W=c["W"],
@@ -99,7 +101,7 @@ def one_case(rng):
         n = len(pd["x"])
         if n == 0:
             break
-        if window and op in ("exec_raise", "exec_mixed"):
+        if window and op in ("exec_raise", "exec_mixed") and not WINDOWED_LISTS:
             continue
         if op == "exec":
             name = str(rng.choice(names3 if three else names2))
@@ -241,8 +243,9 @@ def one_case(rng):
 
 
 def main():
-    n = int(sys.argv[1]) if len(sys.argv) > 1 else 50
-    rng = np.random.default_rng(int(sys.argv[2]) if len(sys.argv) > 2 else 0)
+    args = [a for a in sys.argv[1:] if not a.startswith("--")]
+    n = int(args[0]) if len(args) > 0 else 50
+    rng = np.random.default_rng(int(args[1]) if len(args) > 1 else 0)
     bad = 0
     for k in range(n):
         try:
