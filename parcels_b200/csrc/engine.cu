@@ -24,6 +24,7 @@
 #include <climits>
 #include <cmath>
 #include <cstdarg>
+#include <cstddef>
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
@@ -273,6 +274,39 @@ struct DevBuf {
     }
 };
 
+// The resident particle set: one device column per pointer of ParticlesDev, in its order.  The snapshot keeps whole columns
+// back to back in this order, the ids (when resident) last.
+struct ParticleSoA {
+    struct Column {
+        size_t es;            // bytes per element
+        bool zero_if_absent;  // a NULL host column uploads as zeros (dx, dy, dz)
+        bool optional;        // resident only when the host passes it (particle_id)
+    };
+    static constexpr int NCOL = 10, PID = 9;
+    static constexpr Column cols[NCOL] = {
+        {4, false, false}, {4, false, false}, {4, false, false},  // x y z
+        {4, true, false},  {4, true, false},  {4, true, false},   // dx dy dz
+        {8, false, false}, {4, false, false}, {4, false, false},  // t state ei
+        {8, false, true}};                                        // particle_id
+    static_assert(offsetof(ParticlesDev, n) == NCOL * sizeof(void*), "one column per ParticlesDev pointer");
+    DevBuf col[NCOL];
+
+    // bytes per particle of the snapshot
+    static constexpr size_t row_bytes(bool with_pid) {
+        size_t b = 0;
+        for (const Column& c : cols)
+            if (with_pid || !c.optional) b += c.es;
+        return b;
+    }
+    // particles [lo, lo + n)
+    ParticlesDev view(long long n, long long lo = 0) const {
+        void* c[NCOL];
+        for (int k = 0; k < NCOL; ++k) c[k] = col[k].p ? (char*)col[k].p + (size_t)lo * cols[k].es : nullptr;
+        return ParticlesDev{(float*)c[0], (float*)c[1], (float*)c[2], (float*)c[3], (float*)c[4], (float*)c[5],
+                            (double*)c[6], (int*)c[7], (int*)c[8], (long long*)c[9], n};
+    }
+};
+
 struct pb_engine {
     int device = 0;
     cudaStream_t stream = nullptr;
@@ -305,12 +339,12 @@ struct pb_engine {
     cudaEvent_t copy_done = nullptr;
     std::vector<double> time_host;   // seconds since the interval start
     // particles
-    DevBuf px, py, pz, pdx, pdy, pdz, pt, pstate, pei, ppid;
+    ParticleSoA cur;
     DevBuf snap;  // snapshot of all particle arrays
     long long snap_n = -1;  // particle count the snapshot was taken at (-1: none); a new upload / compaction invalidates it
     bool snap_pid = false;  // the snapshot holds the particle ids too
-    // mode D (domain decomposition): alternate SoA for compaction, migration work buffers
-    DevBuf ax, ay, az, adx, ady, adz, at, astate, aei, apid;
+    // alternate SoA for compaction and migration (rebuild_resident); mode D (domain decomposition) migration work buffers
+    ParticleSoA alt;
     DevBuf mdest, mkeep, mcount, mbounds;
     // output path: block counts / offsets of the ordered selection, selected indices, compacted columns
     DevBuf sblock, soffs, sidx, sout;
@@ -338,10 +372,23 @@ struct pb_engine {
     bool pending = false;
 };
 
-static void zero_report(ReportDev& r) {
+// The bracket of an advect call's launches: a zeroed report and ev0 before them, ev1 and the report's copy back after them;
+// pb_last_report waits for both.
+static int32_t begin_launch(pb_engine* e) {
+    ReportDev& r = *e->h_rep;
     memset(&r, 0, sizeof(r));
     r.first_error_iter = LLONG_MAX;
     r.wait_t_min_bits = ~0ULL;
+    CK(cudaMemcpyAsync(e->d_rep, e->h_rep, sizeof(ReportDev), cudaMemcpyHostToDevice, e->stream));
+    CK(cudaEventRecord(e->ev0, e->stream));
+    return PB_OK;
+}
+
+static int32_t end_launch(pb_engine* e) {
+    CK(cudaEventRecord(e->ev1, e->stream));
+    CK(cudaMemcpyAsync(e->h_rep, e->d_rep, sizeof(ReportDev), cudaMemcpyDeviceToHost, e->stream));
+    e->pending = true;
+    return PB_OK;
 }
 
 // host-side column passes (pb_host_*): a column split over a few C++ threads
@@ -411,14 +458,13 @@ void pb_engine_destroy(pb_engine* e) {
     if (!e) return;
     cudaSetDevice(e->device);
     cudaStreamSynchronize(e->stream);
-    for (DevBuf* b : {&e->ax, &e->ay, &e->az, &e->adx, &e->ady, &e->adz, &e->at, &e->astate, &e->aei, &e->apid, &e->mdest, &e->mkeep,
-                      &e->mcount, &e->mbounds})
-        b->release();
+    for (ParticleSoA* s : {&e->cur, &e->alt})
+        for (DevBuf& b : s->col) b.release();
     for (DevBuf& b : e->fbuf) b.release();
     e->il.release();
-    for (DevBuf* b : {&e->hqbox, &e->hbucket, &e->cellproj, &e->hkeys, &e->hstarts, &e->hcounts, &e->hfaces, &e->lon, &e->lat, &e->depth, &e->time, &e->px, &e->py, &e->pz,
-                      &e->pdx, &e->pdy, &e->pdz, &e->pt, &e->pstate, &e->pei, &e->ppid, &e->snap, &e->sblock, &e->soffs, &e->sidx, &e->sout,
-                      &e->samp_d, &e->samp_i, &e->ad_iters})
+    for (DevBuf* b : {&e->mdest, &e->mkeep, &e->mcount, &e->mbounds, &e->hqbox, &e->hbucket, &e->cellproj, &e->hkeys, &e->hstarts,
+                      &e->hcounts, &e->hfaces, &e->lon, &e->lat, &e->depth, &e->time, &e->snap, &e->sblock, &e->soffs, &e->sidx,
+                      &e->sout, &e->samp_d, &e->samp_i, &e->ad_iters})
         b->release();
     for (int r = 0; r < PB_MIG_MAX_RANKS; ++r)
         if (e->mig_ipc_opened[r]) cudaIpcCloseMemHandle(e->mig_peer[r]);
@@ -690,20 +736,18 @@ int32_t pb_particles_upload(pb_engine* e, int64_t n, const float* x, const float
     if (n < 0) return fail(PB_ERR_INVALID, "n < 0");
     if (n && (!x || !y || !z || !t || !state || !ei)) return fail(PB_ERR_INVALID, "NULL particle array");
     CK(cudaSetDevice(e->device));
-    int32_t rc;
-    if ((rc = upload(e, e->px, x, n * 4))) return rc;
-    if ((rc = upload(e, e->py, y, n * 4))) return rc;
-    if ((rc = upload(e, e->pz, z, n * 4))) return rc;
-    for (auto pr : {std::make_pair(&e->pdx, dx), std::make_pair(&e->pdy, dy), std::make_pair(&e->pdz, dz)}) {
-        if ((rc = pr.first->ensure(n ? n * 4 : 1))) return rc;
-        if (pr.second) { if (n) CK(cudaMemcpyAsync(pr.first->p, pr.second, n * 4, cudaMemcpyHostToDevice, e->stream)); }
-        else if (n) CK(cudaMemsetAsync(pr.first->p, 0, n * 4, e->stream));
-    }
-    if ((rc = upload(e, e->pt, t, n * 8))) return rc;
-    if ((rc = upload(e, e->pstate, state, n * 4))) return rc;
-    if ((rc = upload(e, e->pei, ei, n * 4))) return rc;
+    const void* src[ParticleSoA::NCOL] = {x, y, z, dx, dy, dz, t, state, ei, particle_id};
     e->have_pid = particle_id != nullptr;
-    if (particle_id && (rc = upload(e, e->ppid, particle_id, n * 8))) return rc;
+    for (int k = 0; k < ParticleSoA::NCOL; ++k) {
+        const ParticleSoA::Column& c = ParticleSoA::cols[k];
+        if (c.optional && !src[k]) continue;
+        DevBuf& b = e->cur.col[k];
+        int32_t rc = b.ensure(n ? n * c.es : 1);
+        if (rc) return rc;
+        if (!n) continue;
+        if (src[k]) CK(cudaMemcpyAsync(b.p, src[k], n * c.es, cudaMemcpyHostToDevice, e->stream));
+        else if (c.zero_if_absent) CK(cudaMemsetAsync(b.p, 0, n * c.es, e->stream));
+    }
     e->n = n;
     e->snap_n = -1;
     CK(cudaStreamSynchronize(e->stream));
@@ -716,11 +760,9 @@ int32_t pb_particles_download(pb_engine* e, int64_t n, float* x, float* y, float
     if (!e) return fail(PB_ERR_INVALID, "engine is NULL");
     if (n != e->n) return fail(PB_ERR_INVALID, "download of %lld particles but %lld are resident", (long long)n, (long long)e->n);
     CK(cudaSetDevice(e->device));
-    struct { void* dst; void* src; size_t es; } cp[] = {
-        {x, e->px.p, 4}, {y, e->py.p, 4}, {z, e->pz.p, 4}, {dx, e->pdx.p, 4}, {dy, e->pdy.p, 4}, {dz, e->pdz.p, 4},
-        {t, e->pt.p, 8}, {state, e->pstate.p, 4}, {ei, e->pei.p, 4}};
-    for (auto& c : cp)
-        if (c.dst && n) CK(cudaMemcpyAsync(c.dst, c.src, n * c.es, cudaMemcpyDeviceToHost, e->stream));
+    void* dst[ParticleSoA::PID] = {x, y, z, dx, dy, dz, t, state, ei};  // (the ids: pb_particles_download_ids)
+    for (int k = 0; k < ParticleSoA::PID; ++k)
+        if (dst[k] && n) CK(cudaMemcpyAsync(dst[k], e->cur.col[k].p, n * ParticleSoA::cols[k].es, cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));
     return PB_OK;
 }
@@ -730,29 +772,27 @@ int32_t pb_particles_download_ids(pb_engine* e, int64_t n, int64_t* particle_id)
     if (n != e->n) return fail(PB_ERR_INVALID, "download of %lld ids but %lld particles are resident", (long long)n, (long long)e->n);
     if (!e->have_pid && n) return fail(PB_ERR_STATE, "no particle ids resident");
     CK(cudaSetDevice(e->device));
-    if (n) CK(cudaMemcpyAsync(particle_id, e->ppid.p, n * 8, cudaMemcpyDeviceToHost, e->stream));
+    if (n) CK(cudaMemcpyAsync(particle_id, e->cur.col[ParticleSoA::PID].p, n * 8, cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));
     return PB_OK;
 }
 
-// Snapshot layout: whole columns back to back at offsets that are multiples of the particle count AT SNAPSHOT TIME --
-// x y z dx dy dz (4 B) t (8 B) state ei (4 B) = 40 B per particle, then particle_id (8 B) when ids are resident.
+// Snapshot layout: whole columns back to back in ParticleSoA order, at offsets that are multiples of the particle count AT
+// SNAPSHOT TIME; particle_id (last) only when ids are resident.
 int32_t pb_particles_snapshot(pb_engine* e) {
     PB_RANGE("pb_particles_snapshot");
     if (!e) return fail(PB_ERR_INVALID, "engine is NULL");
     CK(cudaSetDevice(e->device));
     const size_t n = (size_t)e->n;
-    int32_t rc = e->snap.ensure(n ? n * 48 : 1);
+    int32_t rc = e->snap.ensure(n ? n * ParticleSoA::row_bytes(true) : 1);
     if (rc) return rc;
-    char* s = (char*)e->snap.p;
-    struct { void* src; size_t es; } a[] = {{e->px.p, 4}, {e->py.p, 4}, {e->pz.p, 4}, {e->pdx.p, 4}, {e->pdy.p, 4},
-                                            {e->pdz.p, 4}, {e->pt.p, 8}, {e->pstate.p, 4}, {e->pei.p, 4}};
     size_t off = 0;
-    for (auto& c : a) {
-        if (n) CK(cudaMemcpyAsync(s + off, c.src, n * c.es, cudaMemcpyDeviceToDevice, e->stream));
+    for (int k = 0; k < ParticleSoA::NCOL; ++k) {
+        const ParticleSoA::Column& c = ParticleSoA::cols[k];
+        if (c.optional && !e->have_pid) continue;
+        if (n) CK(cudaMemcpyAsync((char*)e->snap.p + off, e->cur.col[k].p, n * c.es, cudaMemcpyDeviceToDevice, e->stream));
         off += n * c.es;
     }
-    if (e->have_pid && n) CK(cudaMemcpyAsync(s + off, e->ppid.p, n * 8, cudaMemcpyDeviceToDevice, e->stream));
     e->snap_n = (long long)n;
     e->snap_pid = e->have_pid;
     return PB_OK;
@@ -764,27 +804,22 @@ int32_t pb_particles_restore(pb_engine* e) {
     PB_RANGE("pb_particles_restore");
     if (!e) return fail(PB_ERR_INVALID, "engine is NULL");
     CK(cudaSetDevice(e->device));
-    if (e->snap_n < 0 || e->snap.bytes < (size_t)e->snap_n * (e->snap_pid ? 48 : 40))
+    if (e->snap_n < 0 || e->snap.bytes < (size_t)e->snap_n * ParticleSoA::row_bytes(e->snap_pid))
         return fail(PB_ERR_STATE, "no snapshot of the resident set to restore (the set was replaced or compacted since pb_particles_snapshot)");
     const size_t n = (size_t)e->snap_n;  // (stream-ordered after a pending advect launch: restore + launch sequences need no host sync)
     if (e->snap_n != e->n && !e->snap_pid)
         return fail(PB_ERR_STATE, "snapshot of %lld particles without ids cannot replace %lld resident ones", e->snap_n, (long long)e->n);
-    char* s = (char*)e->snap.p;
-    struct { DevBuf* dst; size_t es; } a[] = {{&e->px, 4}, {&e->py, 4}, {&e->pz, 4}, {&e->pdx, 4}, {&e->pdy, 4},
-                                              {&e->pdz, 4}, {&e->pt, 8}, {&e->pstate, 4}, {&e->pei, 4}};
     size_t off = 0;
-    for (auto& c : a) {
-        int32_t rc = c.dst->ensure(n ? n * c.es : 1);  // (after a migration the current buffers may be the smaller alternates)
+    for (int k = 0; k < ParticleSoA::NCOL; ++k) {
+        const ParticleSoA::Column& c = ParticleSoA::cols[k];
+        if (c.optional && !e->snap_pid) continue;
+        DevBuf& b = e->cur.col[k];
+        int32_t rc = b.ensure(n ? n * c.es : 1);  // (after a migration the current buffers may be the smaller alternates)
         if (rc) return rc;
-        if (n) CK(cudaMemcpyAsync(c.dst->p, s + off, n * c.es, cudaMemcpyDeviceToDevice, e->stream));
+        if (n) CK(cudaMemcpyAsync(b.p, (char*)e->snap.p + off, n * c.es, cudaMemcpyDeviceToDevice, e->stream));
         off += n * c.es;
     }
-    if (e->snap_pid) {
-        int32_t rc = e->ppid.ensure(n ? n * 8 : 1);
-        if (rc) return rc;
-        if (n) CK(cudaMemcpyAsync(e->ppid.p, s + off, n * 8, cudaMemcpyDeviceToDevice, e->stream));
-        e->have_pid = true;
-    }
+    if (e->snap_pid) e->have_pid = true;
     e->n = (long long)n;
     return PB_OK;
 }
@@ -809,6 +844,20 @@ static void fill_field_desc(pb_engine* e, FieldDev& f) {
     }
 }
 
+// FieldDev of the field in one slot (p[0] only, every level resident), its shape validated against the grid
+static int32_t field_slot_desc(pb_engine* e, int32_t slot, FieldDev& f) {
+    const long long T = e->fshape[slot][0], Z = e->fshape[slot][1], Y = e->fshape[slot][2], X = e->fshape[slot][3];
+    if ((X > 1 && X != e->g.nx) || (Y > 1 && Y != e->g.ny) || (Z > 1 && e->g.nz > 0 && Z != e->g.nz) || (T > 1 && T != e->g.nt))
+        return fail(PB_ERR_INVALID, "field shape (%lld,%lld,%lld,%lld) does not match grid nodes (nt=%d nz=%d ny=%d nx=%d)", T, Z, Y, X,
+                    e->g.nt, e->g.nz, e->g.ny, e->g.nx);
+    if (Z > 1 && e->g.nz == 0) return fail(PB_ERR_INVALID, "field has a depth dimension but the grid has no Z axis");
+    f = FieldDev{};
+    f.p[0] = e->fptr[slot];
+    f.T = (int)T; f.Z = (int)Z; f.Y = (int)Y; f.X = (int)X;
+    f.sX = X > 1 ? 1 : 0; f.sY = Y > 1 ? X : 0; f.sZ = Z > 1 ? X * Y : 0; f.sT = T > 1 ? X * Y * Z : 0;
+    f.ring = (int)T; f.windowed = 0;
+    return PB_OK;
+}
 
 
 // validation shared by pb_advect and pb_sample_velocity; nc = 2 (UV) or 3 (UVW)
@@ -912,14 +961,11 @@ int32_t pb_sample_scalar(pb_engine* e, int32_t slot, int32_t method, int64_t n, 
     if (e->g.curvilinear && method == PB_SCALAR_XLINEAR_INVDIST_LAND)
         return fail(PB_ERR_INVALID, "on curvilinear grids scalar sampling is implemented for XLinear, CGrid_Tracer and XNearest");
     if (e->ring && slot < 3) return fail(PB_ERR_INVALID, "U, V, W are time-windowed: sample them through pb_sample_velocity");
-    const long long T = e->fshape[slot][0], Z = e->fshape[slot][1], Y = e->fshape[slot][2], X = e->fshape[slot][3];
-    if ((X > 1 && X != e->g.nx) || (Y > 1 && Y != e->g.ny) || (Z > 1 && e->g.nz > 0 && Z != e->g.nz) || (T > 1 && T != e->g.nt))
-        return fail(PB_ERR_INVALID, "field shape (%lld,%lld,%lld,%lld) does not match grid nodes (nt=%d nz=%d ny=%d nx=%d)", T, Z, Y, X,
-                    e->g.nt, e->g.nz, e->g.ny, e->g.nx);
-    if (Z > 1 && e->g.nz == 0) return fail(PB_ERR_INVALID, "field has a depth dimension but the grid has no Z axis");
+    SampleParams sp{};
+    int32_t rc = field_slot_desc(e, slot, sp.f);
+    if (rc) return rc;
     if (n == 0) return PB_OK;
     CK(cudaSetDevice(e->device));
-    int32_t rc;
     if ((rc = e->samp_d.ensure((size_t)n * 5 * sizeof(double)))) return rc;
     if ((rc = e->samp_i.ensure(((size_t)n * 4 + 1) * sizeof(int)))) return rc;
     double* d = (double*)e->samp_d.p;  // t z y x value
@@ -927,23 +973,18 @@ int32_t pb_sample_scalar(pb_engine* e, int32_t slot, int32_t method, int64_t n, 
     const double* src[4] = {t, z, y, x};
     for (int k = 0; k < 4; ++k) CK(cudaMemcpyAsync(d + k * n, src[k], n * 8, cudaMemcpyHostToDevice, e->stream));
     if (ei_hint) CK(cudaMemcpyAsync(di, ei_hint, n * 4, cudaMemcpyHostToDevice, e->stream));
-    SampleParams sp{};
     sp.g = e->g;
-    FieldDev& f = sp.f;
-    f.p[0] = e->fptr[slot]; f.p[1] = f.p[2] = nullptr;
-    f.T = (int)T; f.Z = (int)Z; f.Y = (int)Y; f.X = (int)X;
-    f.sX = X > 1 ? 1 : 0; f.sY = Y > 1 ? X : 0; f.sZ = Z > 1 ? X * Y : 0; f.sT = T > 1 ? X * Y * Z : 0;
-    f.ring = (int)T; f.windowed = 0;
     sp.n = n;
     sp.t = d; sp.z = d + n; sp.y = d + 2 * n; sp.x = d + 3 * n;
     sp.u = d + 4 * n; sp.v = nullptr; sp.w = nullptr;
     sp.ei_hint = ei_hint ? di : nullptr;
     sp.ei_out = di + n; sp.state_out = di + 2 * n; sp.f32_out = di + 3 * n;
     sp.pos_f32 = positions_are_f32; sp.no_hint = ei_hint ? 0 : 1;
-    if ((rc = launch_sample_flags(e, sp, T > 1, di + 4 * n))) return rc;
+    const bool has_time = sp.f.T > 1;
+    if ((rc = launch_sample_flags(e, sp, has_time, di + 4 * n))) return rc;
     // a field without a time dimension has no time interval: no time search at all (field.py:112-117)
-    cudaError_t ce = e->g.curvilinear ? launch_sample_scalar_curv(sp, 3 + method, e->coord_f64 != 0, e->f_f64[slot] != 0, T > 1, e->stream)
-                                      : launch_sample_scalar(sp, 3 + method, e->coord_f64 != 0, e->f_f64[slot] != 0, T > 1, e->stream);
+    cudaError_t ce = e->g.curvilinear ? launch_sample_scalar_curv(sp, 3 + method, e->coord_f64 != 0, e->f_f64[slot] != 0, has_time, e->stream)
+                                      : launch_sample_scalar(sp, 3 + method, e->coord_f64 != 0, e->f_f64[slot] != 0, has_time, e->stream);
     if (ce != cudaSuccess) return fail(PB_ERR_CUDA, "sample_kernel launch failed: %s", cudaGetErrorString(ce));
     CK(cudaMemcpyAsync(value, d + 4 * n, n * 8, cudaMemcpyDeviceToHost, e->stream));
     CK(cudaMemcpyAsync(ei_out, di + n, n * 4, cudaMemcpyDeviceToHost, e->stream));
@@ -989,7 +1030,23 @@ static int32_t ensure_interleaved(pb_engine* e, int scheme) {
     return PB_OK;
 }
 
-// validation + kernel parameters shared by pb_advect_async and pb_advect_host (p.P is filled by the caller)
+// kernel parameters every advect entry point takes from the engine and from its arguments (pb_advect_args, pb_rk45_args,
+// pb_advdiff_args); each entry point sets its own on top
+extern "C++" {
+template <class Args>
+static void fill_advect_params(pb_engine* e, const Args* a, AdvectParams& p) {
+    p.g = e->g;
+    fill_field_desc(e, p.f);
+    p.P = e->cur.view(e->n);
+    p.delete_on_error = a->delete_on_error;
+    p.dt = a->dt; p.endtime = a->endtime; p.max_iters = a->max_iters;
+    p.resume = a->resume; p.kernels_only = a->kernels_only;
+    p.batch_levels = a->batch_levels;
+    p.rep = e->d_rep;
+}
+}
+
+// validation + kernel parameters shared by pb_advect_async and pb_advect_host (pb_advect_host sets p.P per chunk)
 static int32_t prepare_advect(pb_engine* e, const pb_advect_args* a, AdvectParams& p, int& nc) {
     if (!e || !a) return fail(PB_ERR_INVALID, "NULL argument");
     if (a->dt == 0.0 || a->dt != a->dt) return fail(PB_ERR_INVALID, "dt must be a non-zero number");
@@ -998,25 +1055,15 @@ static int32_t prepare_advect(pb_engine* e, const pb_advect_args* a, AdvectParam
         case PB_ADVECTION_RK2_3D: case PB_ADVECTION_RK4_3D: nc = 3; break;
         default: return fail(PB_ERR_INVALID, "unknown scheme %d", a->scheme);
     }
-    int32_t rc2;
-    {
-        int32_t rc = check_fields(e, nc);
-        if (rc) return rc;
-    }
-    p.g = e->g;
-    if ((rc2 = ensure_interleaved(e, a->scheme))) return rc2;
-    fill_field_desc(e, p.f);
-    p.scheme = a->scheme; p.diffusion = a->diffusion; p.delete_on_error = a->delete_on_error;
+    int32_t rc = check_fields(e, nc);
+    if (rc) return rc;
+    if ((rc = ensure_interleaved(e, a->scheme))) return rc;  // (before the field descriptor: it may now point at the copy)
+    fill_advect_params(e, a, p);
+    p.scheme = a->scheme; p.diffusion = a->diffusion;
     p.kh_spherical = a->kh_spherical;
-    p.dt = a->dt; p.endtime = a->endtime;
     p.kh_zonal = a->kh_zonal; p.kh_meridional = a->kh_meridional; p.kh_deg2m = a->kh_deg2m;
-    p.seed = a->seed; p.rng_call = a->rng_call; p.max_iters = a->max_iters;
+    p.seed = a->seed; p.rng_call = a->rng_call;
     p.hint_all_zero = a->hint_all_zero;
-    p.resume = a->resume;
-    p.kernels_only = a->kernels_only;
-    p.batch_levels = a->batch_levels;
-    p.g.off_x = e->g.off_x; p.g.off_y = e->g.off_y; p.g.off_z = e->g.off_z;
-    p.rep = e->d_rep;
     if (e->mig_on && e->g.decomposed) {
         if (!e->have_pid) return fail(PB_ERR_STATE, "migration needs particle_id");
         for (int r = 0; r < e->nranks; ++r) p.mig.peer[r] = e->mig_peer[r];
@@ -1051,20 +1098,13 @@ int32_t pb_advect_async(pb_engine* e, const pb_advect_args* a) {
     if (rc) return rc;
     if (a->diffusion && !e->have_pid) return fail(PB_ERR_STATE, "diffusion needs particle_id (RNG counter)");
     CK(cudaSetDevice(e->device));
-    p.P = ParticlesDev{(float*)e->px.p, (float*)e->py.p, (float*)e->pz.p, (float*)e->pdx.p, (float*)e->pdy.p,
-                       (float*)e->pdz.p, (double*)e->pt.p, (int*)e->pstate.p, (int*)e->pei.p, (long long*)e->ppid.p, e->n};
     p.lone_particle = e->n == 1;
-    zero_report(*e->h_rep);
-    CK(cudaMemcpyAsync(e->d_rep, e->h_rep, sizeof(ReportDev), cudaMemcpyHostToDevice, e->stream));
-    CK(cudaEventRecord(e->ev0, e->stream));
+    if ((rc = begin_launch(e))) return rc;
     if (e->n > 0) {
         cudaError_t ce = launch_advect_kernel(e, p, nc, e->stream);
         if (ce != cudaSuccess) return fail(PB_ERR_CUDA, "advect_kernel launch failed: %s", cudaGetErrorString(ce));
     }
-    CK(cudaEventRecord(e->ev1, e->stream));
-    CK(cudaMemcpyAsync(e->h_rep, e->d_rep, sizeof(ReportDev), cudaMemcpyDeviceToHost, e->stream));
-    e->pending = true;
-    return PB_OK;
+    return end_launch(e);
 }
 
 // Kernel.execute on HOST particle arrays, software-pipelined: the set is cut into chunks, each chunk goes H2D -> start-of-interval
@@ -1093,24 +1133,19 @@ int32_t pb_advect_host(pb_engine* e, const pb_advect_args* a, int64_t n, const p
         }
     }
     CK(cudaStreamSynchronize(e->stream));  // the buffers may be re-allocated below: nothing of an earlier call may be in flight
-    struct Col { DevBuf* buf; const void* src; void* dst; size_t es; };
-    Col cols[10] = {{&e->px, h->x, h->x, 4}, {&e->py, h->y, h->y, 4}, {&e->pz, h->z, h->z, 4}, {&e->pdx, h->dx, h->dx, 4},
-                    {&e->pdy, h->dy, h->dy, 4}, {&e->pdz, h->dz, h->dz, 4}, {&e->pt, h->t, h->t, 8},
-                    {&e->pstate, h->state, h->state, 4}, {&e->pei, h->ei, h->ei, 4}, {&e->ppid, h->particle_id, nullptr, 8}};
-    for (int c = 0; c < 10; ++c)
-        if (c < 9 || h->particle_id) {
-            if ((rc = cols[c].buf->ensure(n ? (size_t)n * cols[c].es : 1))) return rc;
-        }
-    if ((rc = e->snap.ensure(n ? (size_t)n * 48 : 1))) return rc;
+    const void* src[ParticleSoA::NCOL] = {h->x, h->y, h->z, h->dx, h->dy, h->dz, h->t, h->state, h->ei, h->particle_id};
+    // the columns this call makes resident and snapshots: all but the ids when none are given
+    auto resident = [&](int k) { return !ParticleSoA::cols[k].optional || src[k]; };
+    for (int k = 0; k < ParticleSoA::NCOL; ++k)
+        if (resident(k) && (rc = e->cur.col[k].ensure(n ? (size_t)n * ParticleSoA::cols[k].es : 1))) return rc;
+    if ((rc = e->snap.ensure(n ? (size_t)n * ParticleSoA::row_bytes(true) : 1))) return rc;
     e->have_pid = h->particle_id != nullptr;
     e->snap_pid = e->have_pid;
     e->n = n;
     e->snap_n = n;  // the chunks below write the start-of-interval copy
     p.lone_particle = n == 1;
 
-    zero_report(*e->h_rep);
-    CK(cudaMemcpyAsync(e->d_rep, e->h_rep, sizeof(ReportDev), cudaMemcpyHostToDevice, e->stream));
-    CK(cudaEventRecord(e->ev0, e->stream));
+    if ((rc = begin_launch(e))) return rc;
     CK(cudaEventRecord(e->pipe_fork, e->stream));
     // chunks of whole waves of 256-thread blocks over the H100's 132 SMs; small sets are not cut
     const long long align = 256 * 132;
@@ -1124,18 +1159,17 @@ int32_t pb_advect_host(pb_engine* e, const pb_advect_args* a, int64_t n, const p
         cudaStream_t st = e->pipe_stream[c % pb_engine::PIPE];
         const long long lo = c * per, m = (n - lo < per ? n - lo : per);
         size_t snap_off = 0;
-        for (int k = 0; k < 10; ++k) {
-            char* dev = (char*)cols[k].buf->p + (size_t)lo * cols[k].es;
-            if (cols[k].src) CK(cudaMemcpyAsync(dev, (const char*)cols[k].src + (size_t)lo * cols[k].es, (size_t)m * cols[k].es, cudaMemcpyHostToDevice, st));
-            else if (k >= 3 && k <= 5) CK(cudaMemsetAsync(dev, 0, (size_t)m * 4, st));  // dx / dy / dz not given: zeros
-            if (k < 9 || cols[k].src) {  // start-of-interval copy in pb_particles_snapshot's layout (whole columns back to back)
-                CK(cudaMemcpyAsync((char*)e->snap.p + snap_off + (size_t)lo * cols[k].es, dev, (size_t)m * cols[k].es, cudaMemcpyDeviceToDevice, st));
-                snap_off += (size_t)n * cols[k].es;
-            }
+        for (int k = 0; k < ParticleSoA::NCOL; ++k) {
+            if (!resident(k)) continue;
+            const ParticleSoA::Column& col = ParticleSoA::cols[k];
+            char* dev = (char*)e->cur.col[k].p + (size_t)lo * col.es;
+            if (src[k]) CK(cudaMemcpyAsync(dev, (const char*)src[k] + (size_t)lo * col.es, (size_t)m * col.es, cudaMemcpyHostToDevice, st));
+            else if (col.zero_if_absent) CK(cudaMemsetAsync(dev, 0, (size_t)m * col.es, st));
+            // start-of-interval copy in pb_particles_snapshot's layout
+            CK(cudaMemcpyAsync((char*)e->snap.p + snap_off + (size_t)lo * col.es, dev, (size_t)m * col.es, cudaMemcpyDeviceToDevice, st));
+            snap_off += (size_t)n * col.es;
         }
-        p.P = ParticlesDev{(float*)e->px.p + lo, (float*)e->py.p + lo, (float*)e->pz.p + lo, (float*)e->pdx.p + lo, (float*)e->pdy.p + lo,
-                           (float*)e->pdz.p + lo, (double*)e->pt.p + lo, (int*)e->pstate.p + lo, (int*)e->pei.p + lo,
-                           e->have_pid ? (long long*)e->ppid.p + lo : (long long*)e->ppid.p, m};
+        p.P = e->cur.view(m, lo);
         cudaError_t ce = launch_advect_kernel(e, p, nc, st);
         if (ce != cudaSuccess) return fail(PB_ERR_CUDA, "advect_kernel launch failed: %s", cudaGetErrorString(ce));
     }
@@ -1143,17 +1177,18 @@ int32_t pb_advect_host(pb_engine* e, const pb_advect_args* a, int64_t n, const p
         for (long long c = 0; c < nchunk; ++c) {
             cudaStream_t st = e->pipe_stream[c % pb_engine::PIPE];
             const long long lo = c * per, m = (n - lo < per ? n - lo : per);
-            for (int k = 0; k < 9; ++k)
-                if (cols[k].dst)
-                    CK(cudaMemcpyAsync((char*)cols[k].dst + (size_t)lo * cols[k].es, (char*)cols[k].buf->p + (size_t)lo * cols[k].es, (size_t)m * cols[k].es, cudaMemcpyDeviceToHost, st));
+            for (int k = 0; k < ParticleSoA::PID; ++k) {  // (the ids are not written back)
+                const size_t es = ParticleSoA::cols[k].es;
+                if (src[k])
+                    CK(cudaMemcpyAsync((char*)const_cast<void*>(src[k]) + (size_t)lo * es, (char*)e->cur.col[k].p + (size_t)lo * es,
+                                       (size_t)m * es, cudaMemcpyDeviceToHost, st));
+            }
         }
     for (int k = 0; k < nstream; ++k) {
         CK(cudaEventRecord(e->pipe_done[k], e->pipe_stream[k]));
         CK(cudaStreamWaitEvent(e->stream, e->pipe_done[k], 0));
     }
-    CK(cudaEventRecord(e->ev1, e->stream));
-    CK(cudaMemcpyAsync(e->h_rep, e->d_rep, sizeof(ReportDev), cudaMemcpyDeviceToHost, e->stream));
-    e->pending = true;
+    if ((rc = end_launch(e))) return rc;
     pb_report tmp;
     rc = pb_last_report(e, &tmp);
     if (rc) return rc;
@@ -1205,8 +1240,6 @@ int32_t pb_advect(pb_engine* e, const pb_advect_args* a, pb_report* rep) {
     return PB_OK;
 }
 
-static ParticlesDev cur_particles(pb_engine* e);
-
 int32_t pb_advect_rk45(pb_engine* e, const pb_rk45_args* a, double* dt_inout, double* next_dt_inout, pb_report* rep) {
     PB_RANGE("pb_advect_rk45");
     if (!e || !a || !rep) return fail(PB_ERR_INVALID, "NULL argument");
@@ -1231,21 +1264,11 @@ int32_t pb_advect_rk45(pb_engine* e, const pb_rk45_args* a, double* dt_inout, do
         CK(cudaMemcpyAsync(d_ndt, next_dt_inout, n * 8, cudaMemcpyHostToDevice, e->stream));
     }
     AdvectParams p{};
-    p.g = e->g;
-    fill_field_desc(e, p.f);
-    p.P = cur_particles(e);
+    fill_advect_params(e, a, p);
     p.scheme = PB_ADVECTION_RK45;
-    p.delete_on_error = a->delete_on_error;
-    p.kernels_only = a->kernels_only; p.resume = a->resume;
-    p.dt = a->dt; p.endtime = a->endtime; p.max_iters = a->max_iters;
     p.hint_all_zero = a->hint_all_zero;
-    p.batch_levels = a->batch_levels;
     p.lone_particle = e->n == 1;
-    p.g.off_x = e->g.off_x; p.g.off_y = e->g.off_y; p.g.off_z = e->g.off_z;
-    p.rep = e->d_rep;
-    zero_report(*e->h_rep);
-    CK(cudaMemcpyAsync(e->d_rep, e->h_rep, sizeof(ReportDev), cudaMemcpyHostToDevice, e->stream));
-    CK(cudaEventRecord(e->ev0, e->stream));
+    if ((rc = begin_launch(e))) return rc;
     if (n) {
         cudaError_t ce = cgrid ? launch_rk45_cgrid(p, d_dt, d_ndt, d_it, a->next_dt_is_f32, a->tol, a->min_dt, a->max_dt, e->coord_f64 != 0,
                                                    e->f_f64[0] != 0, e->stream)
@@ -1255,9 +1278,7 @@ int32_t pb_advect_rk45(pb_engine* e, const pb_rk45_args* a, double* dt_inout, do
                                               e->f_f64[0] != 0, e->g.nt > 0, e->stream);
         if (ce != cudaSuccess) return fail(PB_ERR_CUDA, "rk45_kernel launch failed: %s", cudaGetErrorString(ce));
     }
-    CK(cudaEventRecord(e->ev1, e->stream));
-    CK(cudaMemcpyAsync(e->h_rep, e->d_rep, sizeof(ReportDev), cudaMemcpyDeviceToHost, e->stream));
-    e->pending = true;
+    if ((rc = end_launch(e))) return rc;
     if ((rc = pb_last_report(e, rep))) return rc;
     if (n) {
         // once, after the last launch of the call: a launch that left lanes waiting for the time window is resumed, and the
@@ -1273,20 +1294,10 @@ int32_t pb_advect_rk45(pb_engine* e, const pb_rk45_args* a, double* dt_inout, do
     return PB_OK;
 }
 
-// FieldDev of a scalar field slot (p[0] only); validated against the grid like pb_sample_scalar does
+// FieldDev of a scalar field slot (slots 3.. hold the scalar fields)
 static int32_t scalar_field_desc(pb_engine* e, int32_t slot, FieldDev& f) {
     if (slot < 3 || slot >= PB_MAX_FIELDS || !e->fptr[slot]) return fail(PB_ERR_STATE, "no scalar field in slot %d", slot);
-    const long long T = e->fshape[slot][0], Z = e->fshape[slot][1], Y = e->fshape[slot][2], X = e->fshape[slot][3];
-    if ((X > 1 && X != e->g.nx) || (Y > 1 && Y != e->g.ny) || (Z > 1 && e->g.nz > 0 && Z != e->g.nz) || (T > 1 && T != e->g.nt))
-        return fail(PB_ERR_INVALID, "field shape (%lld,%lld,%lld,%lld) does not match grid nodes (nt=%d nz=%d ny=%d nx=%d)", T, Z, Y, X,
-                    e->g.nt, e->g.nz, e->g.ny, e->g.nx);
-    if (Z > 1 && e->g.nz == 0) return fail(PB_ERR_INVALID, "field has a depth dimension but the grid has no Z axis");
-    f = FieldDev{};
-    f.p[0] = e->fptr[slot];
-    f.T = (int)T; f.Z = (int)Z; f.Y = (int)Y; f.X = (int)X;
-    f.sX = X > 1 ? 1 : 0; f.sY = Y > 1 ? X : 0; f.sZ = Z > 1 ? X * Y : 0; f.sT = T > 1 ? X * Y * Z : 0;
-    f.ring = (int)T; f.windowed = 0;
-    return PB_OK;
+    return field_slot_desc(e, slot, f);
 }
 
 int32_t pb_advect_diffusion_async(pb_engine* e, const pb_advdiff_args* a) {
@@ -1308,34 +1319,22 @@ int32_t pb_advect_diffusion_async(pb_engine* e, const pb_advdiff_args* a) {
         return fail(PB_ERR_INVALID, "Kh_zonal and Kh_meridional must share dtype and time dimension");
     CK(cudaSetDevice(e->device));
     AdvectParams p{};
-    p.g = e->g;
-    fill_field_desc(e, p.f);
-    p.P = cur_particles(e);
-    p.delete_on_error = a->delete_on_error;
-    p.dt = a->dt; p.endtime = a->endtime; p.max_iters = a->max_iters;
+    fill_advect_params(e, a, p);
     p.seed = a->seed; p.rng_call = a->rng_call;
-    p.kernels_only = a->kernels_only; p.resume = a->resume;
-    p.batch_levels = a->batch_levels;
-    p.rep = e->d_rep;
     // time-windowed fields: the lanes' iteration counts survive into the resumed launches (resident fields need none)
     int* iters = nullptr;
     if (e->ring) {
         if ((rc = e->ad_iters.ensure(e->n ? (size_t)e->n * sizeof(int) : 1))) return rc;
         iters = (int*)e->ad_iters.p;
     }
-    zero_report(*e->h_rep);
-    CK(cudaMemcpyAsync(e->d_rep, e->h_rep, sizeof(ReportDev), cudaMemcpyHostToDevice, e->stream));
-    CK(cudaEventRecord(e->ev0, e->stream));
+    if ((rc = begin_launch(e))) return rc;
     if (e->n > 0) {
         cudaError_t ce = launch_advdiff(p, fkz, fkm, a->scheme == PB_ADVDIFF_EM, a->dres, a->deg2m_sq, e->coord_f64 != 0, e->f_f64[0] != 0,
                                         e->f_f64[a->kh_zonal_slot] != 0, e->g.nt > 0, fkz.T > 1, e->interp == PB_INTERP_CGRID_VELOCITY,
                                         iters, e->stream);
         if (ce != cudaSuccess) return fail(PB_ERR_CUDA, "advdiff_kernel launch failed: %s", cudaGetErrorString(ce));
     }
-    CK(cudaEventRecord(e->ev1, e->stream));
-    CK(cudaMemcpyAsync(e->h_rep, e->d_rep, sizeof(ReportDev), cudaMemcpyDeviceToHost, e->stream));
-    e->pending = true;
-    return PB_OK;
+    return end_launch(e);
 }
 
 int32_t pb_advect_diffusion(pb_engine* e, const pb_advdiff_args* a, pb_report* rep) {
@@ -1349,9 +1348,7 @@ static int32_t flag_view(pb_engine* e, double dt, double endtime, int new_state)
     if (!e) return fail(PB_ERR_INVALID, "engine is NULL");
     CK(cudaSetDevice(e->device));
     if (e->n > 0) {
-        ParticlesDev P{(float*)e->px.p, (float*)e->py.p, (float*)e->pz.p, (float*)e->pdx.p, (float*)e->pdy.p,
-                       (float*)e->pdz.p, (double*)e->pt.p, (int*)e->pstate.p, (int*)e->pei.p, (long long*)e->ppid.p, e->n};
-        flag_view_kernel<<<(unsigned)((e->n + 255) / 256), 256, 0, e->stream>>>(P, dt, endtime, new_state);
+        flag_view_kernel<<<(unsigned)((e->n + 255) / 256), 256, 0, e->stream>>>(e->cur.view(e->n), dt, endtime, new_state);
         CK(cudaGetLastError());
     }
     CK(cudaStreamSynchronize(e->stream));
@@ -1434,11 +1431,6 @@ int32_t pb_decomp_set(pb_engine* e, int32_t nranks, int32_t rank, const double* 
     return PB_OK;
 }
 
-static ParticlesDev cur_particles(pb_engine* e) {
-    return ParticlesDev{(float*)e->px.p, (float*)e->py.p, (float*)e->pz.p, (float*)e->pdx.p, (float*)e->pdy.p,
-                        (float*)e->pdz.p, (double*)e->pt.p, (int*)e->pstate.p, (int*)e->pei.p, (long long*)e->ppid.p, e->n};
-}
-
 // ordered selection of the resident particles: indices to e->sidx, count returned
 static int32_t run_select(pb_engine* e, const SelectRule& r, long long* n_sel) {
     CK(cudaSetDevice(e->device));
@@ -1449,7 +1441,7 @@ static int32_t run_select(pb_engine* e, const SelectRule& r, long long* n_sel) {
     if ((rc = e->sblock.ensure((size_t)nb * 4))) return rc;
     if ((rc = e->soffs.ensure((size_t)(nb + 1) * 8))) return rc;
     if ((rc = e->sidx.ensure((size_t)e->n * 8))) return rc;
-    const ParticlesDev P = cur_particles(e);
+    const ParticlesDev P = e->cur.view(e->n);
     sel_count<<<(unsigned)nb, SEL_BLOCK, 0, e->stream>>>(P, r, (unsigned int*)e->sblock.p);
     CK(cudaGetLastError());
     long long* offs = (long long*)e->soffs.p;
@@ -1494,7 +1486,7 @@ int32_t pb_output_gather(pb_engine* e, int64_t n_selected, int64_t* index, float
     float* dx = (float*)(o + m * 16);
     float* dy = dx + m;
     float* dz = dy + m;
-    out_gather<<<(unsigned)((m + 255) / 256), 256, 0, e->stream>>>(cur_particles(e), (const long long*)e->sidx.p, (long long)m,
+    out_gather<<<(unsigned)((m + 255) / 256), 256, 0, e->stream>>>(e->cur.view(e->n), (const long long*)e->sidx.p, (long long)m,
                                                                   x ? dx : nullptr, y ? dy : nullptr, z ? dz : nullptr,
                                                                   t ? dt_ : nullptr, particle_id ? dpid : nullptr);
     CK(cudaGetLastError());
@@ -1508,6 +1500,34 @@ int32_t pb_output_gather(pb_engine* e, int64_t n_selected, int64_t* index, float
     return PB_OK;
 }
 
+// The new resident set, built in the alternate columns: the current rows keep_idx[0..n_keep), then n_in arrival records; the
+// alternates then become current.  headroom: allocate 25 % more than needed (fewer reallocations when the count drifts).
+static int32_t rebuild_resident(pb_engine* e, const long long* keep_idx, long long n_keep, const MigRecord* arrivals, long long n_in,
+                                bool headroom) {
+    const long long n_new = n_keep + n_in;
+    const size_t cap = n_new ? (size_t)n_new : 1;
+    for (int k = 0; k < ParticleSoA::NCOL; ++k) {
+        const size_t bytes = cap * ParticleSoA::cols[k].es;
+        int32_t rc = e->alt.col[k].ensure(headroom ? bytes + bytes / 4 : bytes);
+        if (rc) return rc;
+    }
+    const ParticlesDev dst = e->alt.view(n_new);
+    if (n_keep > 0) {
+        mig_compact<<<(unsigned)((n_keep + 255) / 256), 256, 0, e->stream>>>(e->cur.view(e->n), dst, keep_idx, n_keep);
+        CK(cudaGetLastError());
+    }
+    if (n_in > 0) {
+        mig_unpack<<<(unsigned)((n_in + 255) / 256), 256, 0, e->stream>>>(dst, n_keep, arrivals, n_in);
+        CK(cudaGetLastError());
+    }
+    CK(cudaStreamSynchronize(e->stream));
+    std::swap(e->cur, e->alt);
+    e->n = n_new;
+    if (!e->snap_pid) e->snap_n = -1;  // (a snapshot with ids restores the whole earlier set, count included)
+    e->n_keep = n_new;
+    return PB_OK;
+}
+
 int32_t pb_particles_remove_deleted(pb_engine* e, int64_t* n_left) {
     PB_RANGE("pb_particles_remove_deleted");
     if (!e || !n_left) return fail(PB_ERR_INVALID, "NULL argument");
@@ -1518,23 +1538,7 @@ int32_t pb_particles_remove_deleted(pb_engine* e, int64_t* n_left) {
     if (rc) return rc;
     e->n_selected = -1;
     if (keep == e->n) { *n_left = keep; return PB_OK; }
-    const size_t cap = keep ? (size_t)keep : 1;
-    DevBuf* alt[10] = {&e->ax, &e->ay, &e->az, &e->adx, &e->ady, &e->adz, &e->at, &e->astate, &e->aei, &e->apid};
-    DevBuf* cur[10] = {&e->px, &e->py, &e->pz, &e->pdx, &e->pdy, &e->pdz, &e->pt, &e->pstate, &e->pei, &e->ppid};
-    const size_t es[10] = {4, 4, 4, 4, 4, 4, 8, 4, 4, 8};
-    for (int k = 0; k < 10; ++k)
-        if ((rc = alt[k]->ensure(cap * es[k]))) return rc;
-    ParticlesDev dst{(float*)e->ax.p, (float*)e->ay.p, (float*)e->az.p, (float*)e->adx.p, (float*)e->ady.p, (float*)e->adz.p,
-                     (double*)e->at.p, (int*)e->astate.p, (int*)e->aei.p, (long long*)e->apid.p, keep};
-    if (keep > 0) {
-        mig_compact<<<(unsigned)((keep + 255) / 256), 256, 0, e->stream>>>(cur_particles(e), dst, (const long long*)e->sidx.p, keep);
-        CK(cudaGetLastError());
-    }
-    CK(cudaStreamSynchronize(e->stream));
-    for (int k = 0; k < 10; ++k) std::swap(*cur[k], *alt[k]);
-    e->n = keep;
-    if (!e->snap_pid) e->snap_n = -1;  // (a snapshot with ids restores the whole pre-compaction set, count included)
-    e->n_keep = keep;
+    if ((rc = rebuild_resident(e, (const long long*)e->sidx.p, keep, nullptr, 0, false))) return rc;
     *n_left = keep;
     return PB_OK;
 }
@@ -1551,7 +1555,7 @@ int32_t pb_migrate_count(pb_engine* e, int64_t* counts) {
     if ((rc = e->mcount.ensure((size_t)(nr + 1) * 8))) return rc;
     CK(cudaMemsetAsync(e->mcount.p, 0, (size_t)(nr + 1) * 8, e->stream));
     if (e->n > 0) {
-        mig_classify<<<(unsigned)((e->n + 255) / 256), 256, 0, e->stream>>>(cur_particles(e), (const double*)e->mbounds.p, nr, e->rank,
+        mig_classify<<<(unsigned)((e->n + 255) / 256), 256, 0, e->stream>>>(e->cur.view(e->n), (const double*)e->mbounds.p, nr, e->rank,
                                                                             (int*)e->mdest.p, (unsigned long long*)e->mcount.p);
         CK(cudaGetLastError());
     }
@@ -1578,7 +1582,7 @@ int32_t pb_migrate_pack(pb_engine* e, void* sendbuf_dev, int64_t capacity_record
     int32_t rc;
     if ((rc = e->mkeep.ensure(e->n_keep ? e->n_keep * 8 : 8))) return rc;
     if (e->n > 0) {
-        mig_pack<<<(unsigned)((e->n + 255) / 256), 256, 0, e->stream>>>(cur_particles(e), (const int*)e->mdest.p, nr,
+        mig_pack<<<(unsigned)((e->n + 255) / 256), 256, 0, e->stream>>>(e->cur.view(e->n), (const int*)e->mdest.p, nr,
                                                                         (unsigned long long*)e->mcount.p, (MigRecord*)sendbuf_dev,
                                                                         (long long*)e->mkeep.p);
         CK(cudaGetLastError());
@@ -1591,30 +1595,9 @@ int32_t pb_migrate_unpack(pb_engine* e, const void* recvbuf_dev, int64_t n_in) {
     PB_RANGE("pb_migrate_unpack");
     if (!e || n_in < 0 || (n_in && !recvbuf_dev)) return fail(PB_ERR_INVALID, "bad argument");
     CK(cudaSetDevice(e->device));
-    const long long n_new = e->n_keep + n_in;
-    const size_t cap = n_new ? (size_t)n_new : 1;
-    DevBuf* alt[10] = {&e->ax, &e->ay, &e->az, &e->adx, &e->ady, &e->adz, &e->at, &e->astate, &e->aei, &e->apid};
-    DevBuf* cur[10] = {&e->px, &e->py, &e->pz, &e->pdx, &e->pdy, &e->pdz, &e->pt, &e->pstate, &e->pei, &e->ppid};
-    const size_t es[10] = {4, 4, 4, 4, 4, 4, 8, 4, 4, 8};
-    for (int k = 0; k < 10; ++k) {
-        int32_t rc = alt[k]->ensure(cap * es[k] + (cap * es[k]) / 4);  // 25 % head-room: fewer reallocations
-        if (rc) return rc;
-    }
-    ParticlesDev dst{(float*)e->ax.p, (float*)e->ay.p, (float*)e->az.p, (float*)e->adx.p, (float*)e->ady.p, (float*)e->adz.p,
-                     (double*)e->at.p, (int*)e->astate.p, (int*)e->aei.p, (long long*)e->apid.p, n_new};
-    if (e->n_keep > 0) {
-        mig_compact<<<(unsigned)((e->n_keep + 255) / 256), 256, 0, e->stream>>>(cur_particles(e), dst, (const long long*)e->mkeep.p, e->n_keep);
-        CK(cudaGetLastError());
-    }
-    if (n_in > 0) {
-        mig_unpack<<<(unsigned)((n_in + 255) / 256), 256, 0, e->stream>>>(dst, e->n_keep, (const MigRecord*)recvbuf_dev, n_in);
-        CK(cudaGetLastError());
-    }
-    CK(cudaStreamSynchronize(e->stream));
-    for (int k = 0; k < 10; ++k) std::swap(*cur[k], *alt[k]);
-    e->n = n_new;
-    if (!e->snap_pid) e->snap_n = -1;
-    e->n_send = 0; e->n_keep = n_new;
+    int32_t rc = rebuild_resident(e, (const long long*)e->mkeep.p, e->n_keep, (const MigRecord*)recvbuf_dev, n_in, true);
+    if (rc) return rc;
+    e->n_send = 0;
     return PB_OK;
 }
 
@@ -1692,30 +1675,8 @@ int32_t pb_migrate_p2p_finish(pb_engine* e, int64_t* n_in_out, int64_t* n_now) {
     e->n_selected = -1;
     const unsigned long long arrived = *e->h_mig_count;
     const long long n_in = (long long)(arrived < (unsigned long long)e->mig_cap ? arrived : (unsigned long long)e->mig_cap);
-    if (keep != e->n || n_in > 0) {
-        const long long n_new = keep + n_in;
-        const size_t cap = n_new ? (size_t)n_new : 1;
-        DevBuf* alt[10] = {&e->ax, &e->ay, &e->az, &e->adx, &e->ady, &e->adz, &e->at, &e->astate, &e->aei, &e->apid};
-        DevBuf* cur[10] = {&e->px, &e->py, &e->pz, &e->pdx, &e->pdy, &e->pdz, &e->pt, &e->pstate, &e->pei, &e->ppid};
-        const size_t es[10] = {4, 4, 4, 4, 4, 4, 8, 4, 4, 8};
-        for (int k = 0; k < 10; ++k)
-            if ((rc = alt[k]->ensure(cap * es[k] + (cap * es[k]) / 4))) return rc;
-        ParticlesDev dst{(float*)e->ax.p, (float*)e->ay.p, (float*)e->az.p, (float*)e->adx.p, (float*)e->ady.p, (float*)e->adz.p,
-                         (double*)e->at.p, (int*)e->astate.p, (int*)e->aei.p, (long long*)e->apid.p, n_new};
-        if (keep > 0) {
-            mig_compact<<<(unsigned)((keep + 255) / 256), 256, 0, e->stream>>>(cur_particles(e), dst, (const long long*)e->sidx.p, keep);
-            CK(cudaGetLastError());
-        }
-        if (n_in > 0) {
-            mig_unpack<<<(unsigned)((n_in + 255) / 256), 256, 0, e->stream>>>(dst, keep, mig_records(e->mig_base, slot, e->mig_cap), n_in);
-            CK(cudaGetLastError());
-        }
-        CK(cudaStreamSynchronize(e->stream));
-        for (int k = 0; k < 10; ++k) std::swap(*cur[k], *alt[k]);
-        e->n = n_new;
-        if (!e->snap_pid) e->snap_n = -1;
-        e->n_keep = n_new;
-    }
+    if (keep != e->n || n_in > 0)
+        if ((rc = rebuild_resident(e, (const long long*)e->sidx.p, keep, mig_records(e->mig_base, slot, e->mig_cap), n_in, true))) return rc;
     // this slot is written again two rounds from now, after at least one more barrier: reset its counter now
     CK(cudaMemsetAsync(mig_counter(e->mig_base, slot), 0, 8, e->stream));
     e->mig_slot ^= 1;

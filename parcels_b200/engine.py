@@ -15,6 +15,22 @@ def _report_dict(r: Report) -> dict:
     return {name: getattr(r, name) for name, _ in Report._fields_ if not name.startswith("reserved")}
 
 
+# the resident particle columns in the order of the C-ABI's particle arguments (pb_particles_upload, pb_particle_arrays);
+# "ei" is the engine's one column: the last grid's
+PARTICLE_COLUMNS = ("x", "y", "z", "dx", "dy", "dz", "t", "state", "ei", "particle_id")
+_PARTICLE_DTYPES = {"x": np.float32, "y": np.float32, "z": np.float32, "t": np.float64, "state": np.int32}
+
+
+def _check_particle_dtypes(d: dict):
+    for k, dt in _PARTICLE_DTYPES.items():
+        if d[k].dtype != dt:
+            raise TypeError(f"particle variable {k!r} must be {np.dtype(dt).name} (default Particle), got {d[k].dtype}")
+
+
+def _column_ptrs(d: dict, ei_last: np.ndarray, names=PARTICLE_COLUMNS) -> list:
+    return [ptr(ei_last if k == "ei" else d[k]) for k in names]
+
+
 class Engine:
     def __init__(self, device: int = 0):
         self._lib = _lib.load()
@@ -148,24 +164,12 @@ class Engine:
     # -- particles -----------------------------------------------------------------------------
     def upload_particles(self, d: dict, ei_last: np.ndarray):
         n = d["x"].shape[0]
-        for k, dt in (("x", np.float32), ("y", np.float32), ("z", np.float32), ("t", np.float64), ("state", np.int32)):
-            if d[k].dtype != dt:
-                raise TypeError(f"particle variable {k!r} must be {np.dtype(dt).name} (default Particle), got {d[k].dtype}")
-        check(
-            self._lib.pb_particles_upload(
-                self._h, n, ptr(d["x"]), ptr(d["y"]), ptr(d["z"]), ptr(d["dx"]), ptr(d["dy"]), ptr(d["dz"]), ptr(d["t"]),
-                ptr(d["state"]), ptr(ei_last), ptr(d["particle_id"]),
-            )
-        )  # fmt: skip
+        _check_particle_dtypes(d)
+        check(self._lib.pb_particles_upload(self._h, n, *_column_ptrs(d, ei_last)))
 
     def download_particles(self, d: dict, ei_last: np.ndarray):
         n = d["x"].shape[0]
-        check(
-            self._lib.pb_particles_download(
-                self._h, n, ptr(d["x"]), ptr(d["y"]), ptr(d["z"]), ptr(d["dx"]), ptr(d["dy"]), ptr(d["dz"]), ptr(d["t"]),
-                ptr(d["state"]), ptr(ei_last),
-            )
-        )  # fmt: skip
+        check(self._lib.pb_particles_download(self._h, n, *_column_ptrs(d, ei_last, PARTICLE_COLUMNS[:-1])))  # (ids: download_ids)
 
     def download_ids(self, particle_id: np.ndarray):
         check(self._lib.pb_particles_download_ids(self._h, particle_id.shape[0], ptr(particle_id)))
@@ -259,11 +263,8 @@ class Engine:
         from ._lib import ParticleArrays
 
         n = d["x"].shape[0]
-        for k, dt in (("x", np.float32), ("y", np.float32), ("z", np.float32), ("t", np.float64), ("state", np.int32)):
-            if d[k].dtype != dt:
-                raise TypeError(f"particle variable {k!r} must be {np.dtype(dt).name} (default Particle), got {d[k].dtype}")
-        h = ParticleArrays(*(C.cast(ptr(a), C.c_void_p) for a in (d["x"], d["y"], d["z"], d["dx"], d["dy"], d["dz"], d["t"], d["state"],
-                                                                   ei_last, d["particle_id"])))  # fmt: skip
+        _check_particle_dtypes(d)
+        h = ParticleArrays(*(C.cast(p, C.c_void_p) for p in _column_ptrs(d, ei_last)))
         rep = Report()
         check(self._lib.pb_advect_host(self._h, C.byref(args), n, C.byref(h), int(bool(download)), int(n_chunks), C.byref(rep)))
         return _report_dict(rep)
@@ -363,9 +364,7 @@ class Engine:
 
     def download_all(self, ngrids=1) -> dict:
         """Download the resident particle set (its size may have changed through migration)."""
-        from .particle import create_particle_data
-
-        from .particle import _CORE
+        from .particle import _CORE, create_particle_data
 
         n = self.particle_count()
         if n < (1 << 16):
