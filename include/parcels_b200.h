@@ -150,10 +150,17 @@ int32_t pb_field_clear(pb_engine* e, int32_t slot);
  * wait the same way (RK45: the span [t, t + dt] of the particle's clamped dt; M1 / EM: its time t) and are resumed the
  * same way; a resumed launch (resume = 1 without kernels_only) continues every particle's loop-iteration count, so the
  * result -- the Wiener increments of M1 / EM included -- is the resident one bit for bit.  pb_sample_velocity returns
- * PB_ERR_INVALID when a finite sample time inside the time axis lies outside the resident levels. */
+ * PB_ERR_INVALID when a finite sample time inside the time axis lies outside the resident levels.
+ * Scalar fields (slots 3..) stream the same way.  All windowed slots of one engine share one window_levels and the one
+ * window that pb_field_window_set declares; an engine may window scalar slots only.  pb_sample_scalar on a windowed slot
+ * returns PB_ERR_INVALID for a non-resident sample time as pb_sample_velocity does, and pb_advect_diffusion reads windowed
+ * Kh slots through the window of U, V (which must then be windowed too). */
+/* pb_field_window_create: slot 0 .. PB_MAX_FIELDS - 1; allocates and zeroes window_levels + 1 levels of the slot. */
 int32_t pb_field_window_create(pb_engine* e, int32_t slot, int32_t data_is_f64, int64_t T_total, int64_t Z, int64_t Y,
                                int64_t X, int32_t window_levels);
+/* pb_field_window_load: a slot made by pb_field_window_create (0 .. PB_MAX_FIELDS - 1); level < T_total. */
 int32_t pb_field_window_load(pb_engine* e, int32_t slot, int64_t level, const void* host_level_data);
+/* pb_field_window_set: the window of every windowed slot; first_level + n_levels <= the grid's time levels (nt). */
 int32_t pb_field_window_set(pb_engine* e, int64_t first_level, int64_t n_levels);
 
 /* ---- particles: replaces the SoA dict of create_particle_data (_core/particle.py:182-222)

@@ -896,7 +896,7 @@ __global__ void sample_scalar_curv_kernel(const SampleParams s, int mode /* 3: X
             const bool two_t = has_time && (bf >= 0 ? (bf & 1) != 0 : (tau > 0));
             const bool two_z = g.nz > 0 && (bf >= 0 ? (bf & 2) != 0 : !(zeta <= 0));
             const bool zeta_f32 = f32 && std::is_same<A, float>::value;
-            const long long ot[2] = {wrap_idx(ti, f.T) * f.sT, up_idx(ti, f.T) * f.sT};
+            const long long ot[2] = {tslot(f, wrap_idx(ti, f.T)) * f.sT, tslot(f, up_idx(ti, f.T)) * f.sT};
             const long long oz[2] = {wrap_idx(zi, f.Z) * f.sZ, up_idx(zi, f.Z) * f.sZ};
             const long long oy[2] = {wrap_idx(yi, f.Y) * f.sY, up_idx(yi, f.Y) * f.sY};
             const long long ox[2] = {wrap_idx(xi, f.X) * f.sX, up_idx(xi, f.X) * f.sX};
@@ -935,9 +935,9 @@ __global__ void sample_scalar_curv_kernel(const SampleParams s, int mode /* 3: X
         const long long oz = (long long)min(max(kz, 0), f.Z - 1) * f.sZ, oy = (long long)min(max(ky, 0), f.Y - 1) * f.sY,
                         ox = (long long)min(max(kx, 0), f.X - 1) * f.sX;
         const D* __restrict__ P = (const D*)f.p[0];
-        const D c0 = ldg(P + (long long)min(max(ti, 0), f.T - 1) * f.sT + oz + oy + ox);
+        const D c0 = ldg(P + tslot(f, (long long)min(max(ti, 0), f.T - 1)) * f.sT + oz + oy + ox);
         if (s.batch_flags ? ((*s.batch_flags & 1) != 0) : (tau > 0)) {  // lenT == 2 (the batch's decision, from the pre-pass): linear in time in promote(D, float64)
-            const D c1 = ldg(P + up_idx(ti, f.T) * f.sT + oz + oy + ox);
+            const D c1 = ldg(P + tslot(f, up_idx(ti, f.T)) * f.sT + oz + oy + ox);
             value = (double)c0 * (1 - tau) + (double)c1 * tau;
             value_f32 = false;
         } else {

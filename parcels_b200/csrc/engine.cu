@@ -327,8 +327,9 @@ struct pb_engine {
     DevBuf il;
     bool il_valid = false;
     int last_variant = 0;  // kernel family of the last advect launch: 0 generic, 1 specialised RK4 (afast.cu)
-    // time-slab streaming: ring of (window + 1) levels per component, loads on a dedicated copy stream
+    // time-slab streaming: ring of (window + 1) levels per windowed slot, loads on a dedicated copy stream; one window for all
     int ring = 0;                    // 0: every level resident
+    bool fwin[PB_MAX_FIELDS] = {};   // the slot holds a ring of levels (pb_field_window_create), not the whole field
     long long win_first = 0, win_n = 0;
     cudaStream_t copy_stream = nullptr;
     // pb_advect_host: one in-order stream per chunk slot (H2D -> kernel -> D2H), created on first use
@@ -688,6 +689,7 @@ int32_t pb_set_interpolation(pb_engine* e, int32_t method, int32_t off_x, int32_
 
 static int32_t set_field(pb_engine* e, int32_t slot, const void* dev, int32_t is_f64, int64_t T, int64_t Z, int64_t Y, int64_t X) {
     e->fptr[slot] = dev;
+    e->fwin[slot] = false;
     if (slot < 3) e->il_valid = false;
     e->f_f64[slot] = is_f64 ? 1 : 0;
     e->fshape[slot][0] = T; e->fshape[slot][1] = Z; e->fshape[slot][2] = Y; e->fshape[slot][3] = X;
@@ -724,6 +726,7 @@ int32_t pb_field_clear(pb_engine* e, int32_t slot) {
     if (slot < 0 || slot >= PB_MAX_FIELDS) return fail(PB_ERR_INVALID, "bad field slot %d", slot);
     e->fbuf[slot].release();
     e->fptr[slot] = nullptr;
+    e->fwin[slot] = false;
     if (slot < 3) e->il_valid = false;
     return PB_OK;
 }
@@ -826,6 +829,19 @@ int32_t pb_particles_restore(pb_engine* e) {
 
 int64_t pb_particles_count(pb_engine* e) { return e ? e->n : -1; }
 
+static bool uvw_windowed(const pb_engine* e) { return e->fwin[0] || e->fwin[1] || e->fwin[2]; }
+
+// the time levels a FieldDev can read: its ring and the sample times the resident window covers, or every level
+static void set_window_desc(const pb_engine* e, bool windowed, long long T, FieldDev& f) {
+    f.ring = windowed ? e->ring : (int)T;
+    f.windowed = windowed ? 1 : 0;
+    f.win_t0 = 0.0; f.win_t1 = 0.0;
+    if (windowed && e->win_n > 0 && !e->time_host.empty()) {
+        f.win_t0 = e->time_host[e->win_first];
+        f.win_t1 = e->time_host[e->win_first + e->win_n - 1];
+    }
+}
+
 static void fill_field_desc(pb_engine* e, FieldDev& f) {
     const long long T = e->fshape[0][0], Z = e->fshape[0][1], Y = e->fshape[0][2], X = e->fshape[0][3];
     for (int c = 0; c < 3; ++c) f.p[c] = e->fptr[c];
@@ -834,17 +850,28 @@ static void fill_field_desc(pb_engine* e, FieldDev& f) {
     f.sY = Y > 1 ? X : 0;
     f.sZ = Z > 1 ? X * Y : 0;
     f.sT = T > 1 ? X * Y * Z : 0;
-    f.ring = e->ring ? e->ring : (int)T;
-    f.windowed = e->ring ? 1 : 0;
+    set_window_desc(e, uvw_windowed(e), T, f);
     f.il = (e->il_valid && !e->ring) ? e->il.p : nullptr;
-    f.win_t0 = 0.0; f.win_t1 = 0.0;
-    if (e->ring && e->win_n > 0 && !e->time_host.empty()) {
-        f.win_t0 = e->time_host[e->win_first];
-        f.win_t1 = e->time_host[e->win_first + e->win_n - 1];
-    }
 }
 
-// FieldDev of the field in one slot (p[0] only, every level resident), its shape validated against the grid
+// A sampling call on windowed slots: a finite sample time inside the time axis needs its levels resident (outside the axis is
+// OutsideTimeInterval and reads nothing); otherwise its ring slot may hold another level
+static int32_t check_resident_times(pb_engine* e, int64_t n, const double* t) {
+    if (e->time_host.empty()) return PB_OK;
+    const double ax0 = e->time_host.front(), ax1 = e->time_host.back();
+    const double w0 = e->win_n > 0 ? e->time_host[e->win_first] : 0.0;
+    const double w1 = e->win_n > 0 ? e->time_host[e->win_first + e->win_n - 1] : -1.0;
+    double lo = HUGE_VAL, hi = -HUGE_VAL;
+    for (int64_t k = 0; k < n; ++k)
+        if (t[k] >= ax0 && t[k] <= ax1) { lo = t[k] < lo ? t[k] : lo; hi = t[k] > hi ? t[k] : hi; }
+    if (lo <= hi && !(lo >= w0 && hi <= w1))
+        return fail(PB_ERR_INVALID, "sample times [%.17g, %.17g] are not all inside the resident time levels [%.17g, %.17g]: "
+                                    "pb_field_window_set first", lo, hi, w0, w1);
+    return PB_OK;
+}
+
+// FieldDev of the field in one slot (p[0] only; every level resident, or the ring of a windowed slot), its shape validated
+// against the grid
 static int32_t field_slot_desc(pb_engine* e, int32_t slot, FieldDev& f) {
     const long long T = e->fshape[slot][0], Z = e->fshape[slot][1], Y = e->fshape[slot][2], X = e->fshape[slot][3];
     if ((X > 1 && X != e->g.nx) || (Y > 1 && Y != e->g.ny) || (Z > 1 && e->g.nz > 0 && Z != e->g.nz) || (T > 1 && T != e->g.nt))
@@ -855,7 +882,7 @@ static int32_t field_slot_desc(pb_engine* e, int32_t slot, FieldDev& f) {
     f.p[0] = e->fptr[slot];
     f.T = (int)T; f.Z = (int)Z; f.Y = (int)Y; f.X = (int)X;
     f.sX = X > 1 ? 1 : 0; f.sY = Y > 1 ? X : 0; f.sZ = Z > 1 ? X * Y : 0; f.sT = T > 1 ? X * Y * Z : 0;
-    f.ring = (int)T; f.windowed = 0;
+    set_window_desc(e, e->fwin[slot], T, f);
     return PB_OK;
 }
 
@@ -903,19 +930,7 @@ int32_t pb_sample_velocity(pb_engine* e, int64_t n, const double* t, const doubl
     int32_t rc = check_fields(e, nc);
     if (rc) return rc;
     if (n == 0) return PB_OK;
-    if (e->ring && !e->time_host.empty()) {
-        // time-windowed U, V, W: a finite sample time inside the time axis needs its levels resident (outside the axis is
-        // OutsideTimeInterval and reads nothing); otherwise its ring slot may hold another level
-        const double ax0 = e->time_host.front(), ax1 = e->time_host.back();
-        const double w0 = e->win_n > 0 ? e->time_host[e->win_first] : 0.0;
-        const double w1 = e->win_n > 0 ? e->time_host[e->win_first + e->win_n - 1] : -1.0;
-        double lo = HUGE_VAL, hi = -HUGE_VAL;
-        for (int64_t k = 0; k < n; ++k)
-            if (t[k] >= ax0 && t[k] <= ax1) { lo = t[k] < lo ? t[k] : lo; hi = t[k] > hi ? t[k] : hi; }
-        if (lo <= hi && !(lo >= w0 && hi <= w1))
-            return fail(PB_ERR_INVALID, "sample times [%.17g, %.17g] are not all inside the resident time levels [%.17g, %.17g]: "
-                                        "pb_field_window_set first", lo, hi, w0, w1);
-    }
+    if (uvw_windowed(e) && (rc = check_resident_times(e, n, t))) return rc;
     CK(cudaSetDevice(e->device));
     if ((rc = e->samp_d.ensure((size_t)n * 7 * sizeof(double)))) return rc;
     if ((rc = e->samp_i.ensure(((size_t)n * 3 + 1) * sizeof(int)))) return rc;
@@ -965,6 +980,7 @@ int32_t pb_sample_scalar(pb_engine* e, int32_t slot, int32_t method, int64_t n, 
     int32_t rc = field_slot_desc(e, slot, sp.f);
     if (rc) return rc;
     if (n == 0) return PB_OK;
+    if (e->fwin[slot] && (rc = check_resident_times(e, n, t))) return rc;
     CK(cudaSetDevice(e->device));
     if ((rc = e->samp_d.ensure((size_t)n * 5 * sizeof(double)))) return rc;
     if ((rc = e->samp_i.ensure(((size_t)n * 4 + 1) * sizeof(int)))) return rc;
@@ -1317,6 +1333,9 @@ int32_t pb_advect_diffusion_async(pb_engine* e, const pb_advdiff_args* a) {
     if ((rc = scalar_field_desc(e, a->kh_meridional_slot, fkm))) return rc;
     if (e->f_f64[a->kh_zonal_slot] != e->f_f64[a->kh_meridional_slot] || (fkz.T > 1) != (fkm.T > 1))
         return fail(PB_ERR_INVALID, "Kh_zonal and Kh_meridional must share dtype and time dimension");
+    // a windowed Kh reads the levels of the one engine window, which the kernel's wait test checks through U, V
+    if ((fkz.windowed || fkm.windowed) && !uvw_windowed(e))
+        return fail(PB_ERR_INVALID, "time-windowed Kh_zonal / Kh_meridional need time-windowed U and V");
     CK(cudaSetDevice(e->device));
     AdvectParams p{};
     fill_advect_params(e, a, p);
@@ -1694,7 +1713,7 @@ int32_t pb_migrate_p2p_finish(pb_engine* e, int64_t* n_in_out, int64_t* n_now) {
 int32_t pb_field_window_create(pb_engine* e, int32_t slot, int32_t data_is_f64, int64_t T_total, int64_t Z, int64_t Y, int64_t X,
                                int32_t window_levels) {
     if (!e) return fail(PB_ERR_INVALID, "engine is NULL");
-    if (slot < 0 || slot > 2) return fail(PB_ERR_INVALID, "bad field slot %d", slot);
+    if (slot < 0 || slot >= PB_MAX_FIELDS) return fail(PB_ERR_INVALID, "bad field slot %d", slot);
     if (T_total < 2 || Z < 1 || Y < 1 || X < 1 || window_levels < 2) return fail(PB_ERR_INVALID, "a time window needs >= 2 levels of a time-varying field");
     if (window_levels + 1 > T_total) return fail(PB_ERR_INVALID, "window (%d levels) + 1 prefetch slot exceeds the %lld levels of the field: upload it whole", window_levels, (long long)T_total);
     if (e->ring && e->ring != window_levels + 1) return fail(PB_ERR_INVALID, "all components must use the same window");
@@ -1709,13 +1728,15 @@ int32_t pb_field_window_create(pb_engine* e, int32_t slot, int32_t data_is_f64, 
     CK(cudaStreamSynchronize(e->stream));  // the level loads run on the copy stream: the zeros must be in place first
     e->ring = window_levels + 1;
     e->win_first = 0; e->win_n = 0;
-    return set_field(e, slot, e->fbuf[slot].p, data_is_f64, T_total, Z, Y, X);
+    rc = set_field(e, slot, e->fbuf[slot].p, data_is_f64, T_total, Z, Y, X);
+    e->fwin[slot] = true;
+    return rc;
 }
 
 int32_t pb_field_window_load(pb_engine* e, int32_t slot, int64_t level, const void* host_level_data) {
     PB_RANGE("pb_field_window_load");
     if (!e || !host_level_data) return fail(PB_ERR_INVALID, "NULL argument");
-    if (slot < 0 || slot > 2 || !e->ring || !e->fptr[slot]) return fail(PB_ERR_STATE, "pb_field_window_create first");
+    if (slot < 0 || slot >= PB_MAX_FIELDS || !e->fwin[slot]) return fail(PB_ERR_STATE, "pb_field_window_create first");
     if (level < 0 || level >= e->fshape[slot][0]) return fail(PB_ERR_INVALID, "time level %lld out of range", (long long)level);
     CK(cudaSetDevice(e->device));
     const size_t level_bytes = (size_t)e->fshape[slot][1] * e->fshape[slot][2] * e->fshape[slot][3] * (e->f_f64[slot] ? 8 : 4);
@@ -1727,7 +1748,7 @@ int32_t pb_field_window_load(pb_engine* e, int32_t slot, int64_t level, const vo
 int32_t pb_field_window_set(pb_engine* e, int64_t first_level, int64_t n_levels) {
     if (!e) return fail(PB_ERR_INVALID, "engine is NULL");
     if (!e->ring) return fail(PB_ERR_STATE, "pb_field_window_create first");
-    if (first_level < 0 || n_levels < 2 || n_levels > e->ring || first_level + n_levels > e->fshape[0][0])
+    if (first_level < 0 || n_levels < 2 || n_levels > e->ring || first_level + n_levels > e->g.nt)
         return fail(PB_ERR_INVALID, "bad window [%lld, +%lld)", (long long)first_level, (long long)n_levels);
     CK(cudaSetDevice(e->device));
     // the advection stream must not start before the pending level loads have landed

@@ -152,7 +152,7 @@ class Field:
     """Scalar field on the fieldset's grid (reference ``_core/field.py:46-202``).  ``interp_method``: "linear" (XLinear),
     "nearest" (XNearest), "cgrid_tracer" (CGrid_Tracer) or "constant" (XConstantField, a 1-node grid)."""
 
-    def __init__(self, name, data, grid, fieldset, interp_method="linear", slot=None, host=None):
+    def __init__(self, name, data, grid, fieldset, interp_method="linear", slot=None, host=None, windowed=False):
         self.name = name
         self.data = data
         self.grid = grid
@@ -160,6 +160,7 @@ class Field:
         self._host = host  # who keeps this field's grid in HBM: the FieldSet (None) or an _ExtraGrid of it
         self.interp_method = interp_method
         self._slot = slot  # device field slot (include/parcels_b200.h: 0..2 = U, V, W; 3.. = scalar fields)
+        self._windowed = windowed  # only the host's time window of `data`'s levels is in HBM (time-slab streaming)
 
     def eval(self, t, z, y, x, particles=None, *, device=None, positions_are_f32=None):
         """``fieldset.P.eval(t, z, y, x[, particles])`` (reference _core/field.py:144-191), evaluated ON THE DEVICE
@@ -192,8 +193,11 @@ class Field:
         host = self._host or fs
         if _batch_skips_hint(self.grid, hint):
             hint = None
-        val, ei, st = host.engine(device).sample_scalar(self._slot, self.interp_method, t, z, y, x,
-                                                        positions_are_f32=positions_are_f32, ei_hint=hint)  # fmt: skip
+        eng = host.engine(device)
+        if self._windowed:
+            host.cover_window(device, t)  # the batch's levels resident (times outside the axis: OutsideTimeInterval)
+        val, ei, st = eng.sample_scalar(self._slot, self.interp_method, t, z, y, x, positions_are_f32=positions_are_f32,
+                                        ei_hint=hint)  # fmt: skip
         if particles is not None:
             particles.ei[:, -1] = ei
             state = np.asarray(particles.state)
@@ -236,8 +240,8 @@ class VectorField:
         if particles is not None:
             hint = np.ascontiguousarray(np.asarray(particles.ei)[:, -1])
         eng = host.engine(device)
-        if host is fs and fs.time_window is not None:
-            fs.cover_window(device, t)  # time-windowed U, V, W: the batch's levels resident (times outside the axis: OutsideTimeInterval)
+        if self.U._windowed:
+            host.cover_window(device, t)  # time-windowed U, V, W: the batch's levels resident (times outside the axis: OutsideTimeInterval)
         u, v, w, ei, st = eng.sample_velocity(t, z, y, x, three_d=self.W is not None, positions_are_f32=positions_are_f32,
                                                               ei_hint=hint, no_hint=_batch_skips_hint(self.grid, hint))  # fmt: skip
         if particles is not None:
@@ -261,17 +265,114 @@ class VectorField:
         return self.eval(*key)
 
 
-class _ExtraGrid:
+def _field_data(name, data, time_window):
+    """The data of a scalar field: a float32 / float64 (T, Z, Y, X) array uploaded whole, or with ``time_window`` the caller's
+    array-like (np.memmap, a lazy loader ...) itself, of which only ``data[level]`` is ever read."""
+    if time_window is None:
+        data = np.ascontiguousarray(data)
+        if data.ndim != 4:
+            raise ValueError(f"{name} must be laid out (T, Z, Y, X); got shape {data.shape}")
+        return data if data.dtype in (np.float32, np.float64) else data.astype(np.float64)
+    shape = tuple(data.shape)
+    if len(shape) != 4:
+        raise ValueError(f"{name} must be laid out (T, Z, Y, X); got shape {shape}")
+    if np.dtype(data.dtype) not in (np.float32, np.float64):
+        raise ValueError(f"{name}: a time-windowed field must be float32 or float64, got {data.dtype}")
+    if shape[0] < 2:
+        raise ValueError(f"{name} has a single time level: there is no time dimension to stream (add it without time_window)")
+    return data
+
+
+class _TimeWindow:
+    """Time-slab streaming of the windowed fields of one device engine per device (the FieldSet's velocity grid, or an
+    _ExtraGrid): ``time_window`` consecutive levels of the time axis ``_time_s`` resident, plus one ring slot that receives the
+    next level.  The owner has ``_engines``, ``_win`` (device -> window state) and ``_windowed_fields()`` -> [(slot, data)]."""
+
+    def _load_level(self, eng, device, level):
+        w = self._win[device]
+        ring = self.time_window + 1
+        w["resident"] = {lv for lv in w["resident"] if lv % ring != level % ring}
+        for slot, data in self._windowed_fields():
+            eng.window_load(slot, level, np.asarray(data[level]))
+        w["resident"].add(level)
+
+    def _window_add_field(self, slot, data):
+        """A windowed field added after the engines were made: its ring on each, holding the levels resident there."""
+        for device, eng in self._engines.items():
+            eng.window_create(slot, data.dtype, data.shape, self.time_window)
+            w = self._win[device]
+            for lv in sorted(w["resident"]):
+                eng.window_load(slot, lv, np.asarray(data[lv]))
+            if w["n"]:
+                eng.window_set(w["first"], w["n"])
+
+    def slide_window(self, device, t, sign):
+        """Make the levels a particle at time ``t`` needs resident; returns True if the window moved."""
+        return self._set_window(device, *window_range(self._time_s, t, sign, self.time_window))
+
+    def cover_window(self, device, t, sign=1):
+        """Make the levels of every finite sample time in ``t`` that lies inside the time axis resident (a step-by-step kernel
+        list, a user kernel's ``fieldset.UV[...]``).  Raises RuntimeError when no window of ``time_window`` levels holds them."""
+        t = np.asarray(t, dtype=np.float64)
+        inside = t[(t >= self._time_s[0]) & (t <= self._time_s[-1])]  # (NaN fails both tests)
+        if inside.size == 0:
+            return
+        lo, hi = float(inside.min()), float(inside.max())
+        w = self._win[device]
+        if w["n"] and self._time_s[w["first"]] <= lo and hi <= self._time_s[w["first"] + w["n"] - 1]:
+            return
+        span = window_span(self._time_s, lo, hi, sign, self.time_window)
+        if span is None:
+            raise RuntimeError(f"sample times {lo} .. {hi} span more than the {self.time_window} resident time levels of this "
+                               "FieldSet: widen time_window")  # fmt: skip
+        self._set_window(device, *span)
+
+    def _set_window(self, device, first, n):
+        eng = self._engines[device]
+        w = self._win[device]
+        moved = (first, n) != (w["first"], w["n"])
+        for lv in range(first, first + n):
+            if lv not in w["resident"]:
+                self._load_level(eng, device, lv)
+        eng.window_set(first, n)
+        w["first"], w["n"] = first, n
+        return moved
+
+    def prefetch_next(self, device, sign):
+        """Start copying the level the next window will need into the spare ring slot (overlaps the kernel)."""
+        w = self._win[device]
+        nxt = w["first"] + w["n"] if sign > 0 else w["first"] - 1
+        if 0 <= nxt < len(self._time_s) and nxt not in w["resident"]:
+            self._load_level(self._engines[device], device, nxt)
+
+
+class _ExtraGrid(_TimeWindow):
     """A further XGrid of the FieldSet (reference: every Field carries its own grid, _core/field.py:102-134; the gridset is the
     list of distinct grids, _core/fieldset.py:225-235) with the scalar fields that live on it.  Each grid is resident in its own
-    device engine (grid axes / spatial hash + field slots 3..15); the advection kernels only ever see the velocity grid."""
+    device engine (grid axes / spatial hash + field slots 3..15); the advection kernels only ever see the velocity grid.
+    Fields added with ``time_window=W`` stream through one window of W levels over this grid's time axis, slid by the
+    ``eval`` of its fields."""
 
     def __init__(self, grid, time_s):
-        self.grid, self.time_s = grid, time_s
+        self.grid, self._time_s = grid, time_s
         self.fields = []
         self.vector = None  # (U, V, W or None) Field objects of a vector field on this grid: device slots 0..2
         self.vector_interp, self.offsets = None, (1, 1, 0)
+        self.time_window = None  # levels resident of the windowed fields (one window for all of them)
         self._engines = {}
+        self._win = {}
+
+    def _windowed_fields(self):
+        return [(f._slot, f.data) for f in (*(self.vector or ()), *self.fields) if f is not None and f._windowed]
+
+    def use_window(self, name, time_window):
+        """Check ``time_window=`` of a field added to this grid: one window for every windowed field of the grid."""
+        if self._time_s is None:
+            raise ValueError(f"{name}: time_window on a grid without a time axis (no time dimension to stream)")
+        time_window = int(time_window)
+        if self.time_window is not None and time_window != self.time_window:
+            raise ValueError(f"{name}: time_window={time_window}, but the windowed fields of its grid use {self.time_window}")
+        self.time_window = time_window
 
     def engine(self, device: int = 0) -> Engine:
         eng = self._engines.get(device)
@@ -279,16 +380,17 @@ class _ExtraGrid:
             eng = Engine(device)
             g = self.grid
             if g.curvilinear:
-                eng.upload_curvilinear_grid(g.lon, g.lat, g.depth, self.time_s, g.is_spherical(), g.deg2m, g.xdim, g.ydim, g.zdim,
+                eng.upload_curvilinear_grid(g.lon, g.lat, g.depth, self._time_s, g.is_spherical(), g.deg2m, g.xdim, g.ydim, g.zdim,
                                             g.get_spatial_hash())  # fmt: skip
             else:
-                eng.upload_rectilinear_grid(g.lon, g.lat, g.depth, self.time_s, g.is_spherical(), g.deg2m, g.xdim, g.ydim, g.zdim)
+                eng.upload_rectilinear_grid(g.lon, g.lat, g.depth, self._time_s, g.is_spherical(), g.deg2m, g.xdim, g.ydim, g.zdim)
             eng.set_interpolation(INTERP_METHODS[self.vector_interp or ("cgrid_velocity" if g.curvilinear else "linear")], *self.offsets)
-            for slot, f in enumerate(self.vector or ()):
-                if f is not None:
-                    eng.upload_field(slot, f.data)
-            for f in self.fields:
-                eng.upload_field(f._slot, f.data)
+            for f in (*(self.vector or ()), *self.fields):
+                if f is not None and f._windowed:
+                    eng.window_create(f._slot, f.data.dtype, f.data.shape, self.time_window)
+                elif f is not None:
+                    eng.upload_field(f._slot, f.data)
+            self._win[device] = dict(first=0, n=0, resident=set())
             self._engines[device] = eng
         return eng
 
@@ -317,7 +419,7 @@ class _ConstantGrid:
 INTERP_METHODS = {"linear": 0, "cgrid_velocity": 1, "freeslip": 2, "partialslip": 3, "nearest": 4}
 
 
-class FieldSet:
+class FieldSet(_TimeWindow):
     """Velocity fields U, V (, W) laid out (T, Z, Y, X) on one A-grid, plus constant fields.
 
     Build with :meth:`from_arrays` (NumPy arrays) or ``parcels_b200.adapter.from_parcels`` (a
@@ -351,7 +453,8 @@ class FieldSet:
                 arr = np.asarray(arr)
             if len(arr.shape) != 4:
                 raise ValueError(f"{name} must be laid out (T, Z, Y, X); got shape {arr.shape}")
-            self.fields[name] = Field(name, arr, grid, self, slot={"U": 0, "V": 1, "W": 2}[name] if self.time_window is None else None)
+            self.fields[name] = Field(name, arr, grid, self, slot={"U": 0, "V": 1, "W": 2}[name] if self.time_window is None else None,
+                                      windowed=self.time_window is not None)  # fmt: skip
         self.U, self.V, self.W = self.fields["U"], self.fields["V"], self.fields.get("W")
         self.UV = VectorField("UV", self.U, self.V)
         self.fields["UV"] = self.UV
@@ -396,12 +499,17 @@ class FieldSet:
         self.fields[name] = f
         setattr(self, name, f)
 
-    def add_field(self, name, data, interp_method="linear", grid=None, time=None):
+    def add_field(self, name, data, interp_method="linear", grid=None, time=None, time_window=None):
         """Scalar field -- in the reference every data variable of the model's dataset is a ``Field`` with its own ``grid`` and
         ``interp_method`` (_core/fieldset.py:89-108, _core/field.py:102-134); here it is added from an array laid out
         (T, Z, Y, X) with T == the time axis, or T == 1 for a field without a time dimension.  ``grid``: an ``XGrid`` other than
         the velocity grid (a second entry of ``fieldset.gridset``; ``time`` = that field's own time axis, default: the
-        fieldset's).  Sampled on the device: ``fieldset.<name>[particles]`` / ``.eval(t, z, y, x)``."""
+        fieldset's).  Sampled on the device: ``fieldset.<name>[particles]`` / ``.eval(t, z, y, x)``.
+
+        ``time_window=W``: time-slab streaming of this time-varying field -- ``data`` stays the caller's array-like (np.memmap,
+        a lazy loader ...) and only ``data[level]`` of the levels entering the window is read.  On the velocity grid W must be
+        the FieldSet's ``time_window`` (the field rides on the velocity window); on another grid every windowed field of that
+        grid uses one W over the grid's own time axis, slid by the ``eval`` of its fields.  None: the field is uploaded whole."""
         from .engine import Engine
 
         if interp_method not in Engine.SCALAR_METHODS:
@@ -409,36 +517,36 @@ class FieldSet:
         if name in self.fields:
             raise ValueError(f"FieldSet already has a Field with name '{name}'")
         if grid is not None and grid is not self.grid:
-            return self._add_field_on_grid(name, data, interp_method, grid, time)
+            return self._add_field_on_grid(name, data, interp_method, grid, time, time_window)
         if self.grid.curvilinear and interp_method not in ("linear", "nearest", "cgrid_tracer"):
             raise NotImplementedError("on curvilinear grids scalar fields are sampled with 'linear' (XLinear), 'cgrid_tracer' (CGrid_Tracer) "
                                       "or 'nearest' (XNearest)")
-        data = np.ascontiguousarray(data)
-        if data.ndim != 4:
-            raise ValueError(f"{name} must be laid out (T, Z, Y, X); got shape {data.shape}")
-        if data.dtype not in (np.float32, np.float64):
-            data = data.astype(np.float64)
+        if time_window is not None and self.time_window is None:
+            raise ValueError(f"{name}: time_window on a FieldSet built without one (FieldSet.from_arrays(..., time_window=W))")
+        if time_window is not None and int(time_window) != self.time_window:
+            raise ValueError(f"{name}: time_window={time_window}, but a field on the velocity grid streams through the "
+                             f"FieldSet's window of {self.time_window} levels")  # fmt: skip
+        data = _field_data(name, data, time_window)
         nt = 1 if self._time_s is None else self._time_s.size
-        if data.shape[0] not in (1, nt) or data.shape[1:] != self.U.data.shape[1:]:
+        if data.shape[0] not in (1, nt) or tuple(data.shape[1:]) != tuple(self.U.data.shape[1:]):
             raise ValueError(f"{name} has shape {data.shape}; expected ({nt} or 1, {', '.join(map(str, self.U.data.shape[1:]))})")
         slot = 3 + sum(1 for f in self.fields.values() if isinstance(f, Field) and f._host is None and f._slot is not None and f._slot >= 3)
-        f = Field(name, data, self.grid, self, interp_method=interp_method, slot=slot)
+        f = Field(name, data, self.grid, self, interp_method=interp_method, slot=slot, windowed=time_window is not None)
         self.fields[name] = f
         setattr(self, name, f)
-        for eng in self._engines.values():
-            eng.upload_field(slot, data)
+        if f._windowed:
+            self._window_add_field(slot, data)
+        else:
+            for eng in self._engines.values():
+                eng.upload_field(slot, data)
         return f
 
-    def _add_field_on_grid(self, name, data, interp_method, grid, time):
+    def _add_field_on_grid(self, name, data, interp_method, grid, time, time_window):
         if not isinstance(grid, XGrid):
             raise TypeError(f"grid must be an XGrid, got {type(grid).__name__}")
         if grid.curvilinear and interp_method not in ("linear", "nearest", "cgrid_tracer"):
             raise NotImplementedError("on curvilinear grids scalar fields are sampled with 'linear', 'cgrid_tracer' or 'nearest'")
-        data = np.ascontiguousarray(data)
-        if data.ndim != 4:
-            raise ValueError(f"{name} must be laid out (T, Z, Y, X); got shape {data.shape}")
-        if data.dtype not in (np.float32, np.float64):
-            data = data.astype(np.float64)
+        data = _field_data(name, data, time_window)
         time_s = self._time_s if time is None else _to_seconds(time)[0]
         nt = 1 if time_s is None else time_s.size
         nz = 1 if grid.depth is None else len(grid.depth)
@@ -449,23 +557,31 @@ class FieldSet:
         if host is None:
             host = _ExtraGrid(grid, time_s)
             self._extra_grids.append(host)
-        elif (host.time_s is None) != (time_s is None) or (time_s is not None and not np.array_equal(host.time_s, time_s)):
+        elif (host._time_s is None) != (time_s is None) or (time_s is not None and not np.array_equal(host._time_s, time_s)):
             raise NotImplementedError("fields on one grid share one time axis")
         if len(host.fields) >= 13:
             raise NotImplementedError("at most 13 scalar fields per grid")
-        f = Field(name, data, grid, self, interp_method=interp_method, slot=3 + len(host.fields), host=host)
+        if time_window is not None:
+            host.use_window(name, time_window)
+        f = Field(name, data, grid, self, interp_method=interp_method, slot=3 + len(host.fields), host=host,
+                  windowed=time_window is not None)  # fmt: skip
         host.fields.append(f)
         self.fields[name] = f
         setattr(self, name, f)
-        for eng in host._engines.values():
-            eng.upload_field(f._slot, data)
+        if f._windowed:
+            host._window_add_field(f._slot, data)
+        else:
+            for eng in host._engines.values():
+                eng.upload_field(f._slot, data)
         return f
 
-    def add_vector_field(self, name, U, V, W=None, *, grid, interp_method="linear", padding=("low", "low", "high"), time=None):
+    def add_vector_field(self, name, U, V, W=None, *, grid, interp_method="linear", padding=("low", "low", "high"), time=None,
+                         time_window=None):  # fmt: skip
         """A further VectorField on ANOTHER XGrid of the FieldSet (reference: any ``VectorField(name, U, V[, W])`` of the fieldset,
         e.g. a wind field on the atmospheric model's grid, _core/field.py:205-248), for sampling in user kernels --
         ``fieldset.<name>[particles]`` / ``.eval(t, z, y, x)`` -> (u, v[, w]) in the units ``fieldset.UV`` gives (degrees per second on
-        a spherical mesh).  The advection kernels keep using ``fieldset.UV`` / ``UVW`` on the velocity grid."""
+        a spherical mesh).  The advection kernels keep using ``fieldset.UV`` / ``UVW`` on the velocity grid.
+        ``time_window=W``: the components stream through the grid's window of W levels, as in :meth:`add_field`."""
         if not isinstance(grid, XGrid) or grid is self.grid:
             raise ValueError("add_vector_field needs an XGrid other than the velocity grid (fieldset.UV is the vector field of that one)")
         if name in self.fields:
@@ -481,15 +597,21 @@ class FieldSet:
             raise NotImplementedError("one vector field per grid")
         elif host._engines:
             raise NotImplementedError("add the vector field of a grid before its fields are first sampled")
+        if time_window is not None:
+            host.use_window(name, time_window)
         comps = []
         for cname, arr in (("U", U), ("V", V), ("W", W)):
             if arr is None:
                 comps.append(None)
                 continue
-            arr = np.ascontiguousarray(arr)
-            if arr.ndim != 4 or arr.dtype not in (np.float32, np.float64):
-                raise ValueError(f"{name}.{cname} must be a float32 / float64 array laid out (T, Z, Y, X)")
-            comps.append(Field(f"{name}_{cname}", arr, grid, self, interp_method="linear", slot=len(comps), host=host))
+            if time_window is not None:
+                _field_data(f"{name}.{cname}", arr, time_window)
+            else:
+                arr = np.ascontiguousarray(arr)
+                if arr.ndim != 4 or arr.dtype not in (np.float32, np.float64):
+                    raise ValueError(f"{name}.{cname} must be a float32 / float64 array laid out (T, Z, Y, X)")
+            comps.append(Field(f"{name}_{cname}", arr, grid, self, interp_method="linear", slot=len(comps), host=host,
+                               windowed=time_window is not None))  # fmt: skip
         host.vector, host.vector_interp = tuple(comps), interp_method
         host.offsets = tuple(int(p == "low") for p in padding)
         vf = VectorField(name, comps[0], comps[1], comps[2], host=host)
@@ -539,59 +661,19 @@ class FieldSet:
                         eng.window_create(slot, d.dtype, d.shape, self.time_window)
             for f in self.fields.values():
                 if isinstance(f, Field) and f._host is None and f._slot is not None and f._slot >= 3:
-                    eng.upload_field(f._slot, f.data)
+                    if f._windowed:
+                        eng.window_create(f._slot, f.data.dtype, f.data.shape, self.time_window)
+                    else:
+                        eng.upload_field(f._slot, f.data)
             self._win[device] = dict(first=0, n=0, resident=set())
             self._engines[device] = eng
         return eng
 
-    # -- time-slab streaming ---------------------------------------------------------------------------
-    def _load_level(self, eng, device, level):
-        w = self._win[device]
-        ring = self.time_window + 1
-        w["resident"] = {lv for lv in w["resident"] if lv % ring != level % ring}
-        for slot, name in enumerate(("U", "V", "W")):
-            if name in self.fields:
-                eng.window_load(slot, level, np.asarray(self.fields[name].data[level]))
-        w["resident"].add(level)
-
-    def slide_window(self, device, t, sign):
-        """Make the levels a particle at time ``t`` needs resident; returns True if the window moved."""
-        return self._set_window(device, *window_range(self._time_s, t, sign, self.time_window))
-
-    def cover_window(self, device, t, sign=1):
-        """Make the levels of every finite sample time in ``t`` that lies inside the time axis resident (a step-by-step kernel
-        list, a user kernel's ``fieldset.UV[...]``).  Raises RuntimeError when no window of ``time_window`` levels holds them."""
-        t = np.asarray(t, dtype=np.float64)
-        inside = t[(t >= self._time_s[0]) & (t <= self._time_s[-1])]  # (NaN fails both tests)
-        if inside.size == 0:
-            return
-        lo, hi = float(inside.min()), float(inside.max())
-        w = self._win[device]
-        if w["n"] and self._time_s[w["first"]] <= lo and hi <= self._time_s[w["first"] + w["n"] - 1]:
-            return
-        span = window_span(self._time_s, lo, hi, sign, self.time_window)
-        if span is None:
-            raise RuntimeError(f"sample times {lo} .. {hi} span more than the {self.time_window} resident time levels of this "
-                               "FieldSet: widen time_window")  # fmt: skip
-        self._set_window(device, *span)
-
-    def _set_window(self, device, first, n):
-        eng = self._engines[device]
-        w = self._win[device]
-        moved = (first, n) != (w["first"], w["n"])
-        for lv in range(first, first + n):
-            if lv not in w["resident"]:
-                self._load_level(eng, device, lv)
-        eng.window_set(first, n)
-        w["first"], w["n"] = first, n
-        return moved
-
-    def prefetch_next(self, device, sign):
-        """Start copying the level the next window will need into the spare ring slot (overlaps the kernel)."""
-        w = self._win[device]
-        nxt = w["first"] + w["n"] if sign > 0 else w["first"] - 1
-        if 0 <= nxt < len(self._time_s) and nxt not in w["resident"]:
-            self._load_level(self._engines[device], device, nxt)
+    # -- time-slab streaming (_TimeWindow): U, V, W and the scalar fields added with time_window ------------------------------
+    def _windowed_fields(self):
+        uvw = [(slot, self.fields[name].data) for slot, name in enumerate(("U", "V", "W")) if name in self.fields]
+        return uvw + [(f._slot, f.data) for f in self.fields.values() if isinstance(f, Field) and f._host is None and f._slot is not None
+                      and f._slot >= 3 and f._windowed]  # fmt: skip
 
     def release(self):
         for e in self._engines.values():

@@ -645,6 +645,9 @@ class ParticleSet:
         if d["ei"].shape[1] > 1:
             d["ei"][:, 1:] = 0
         for k, host in enumerate(self.fieldset._extra_grids, start=1):  # further XGrids: the search of one of their fields
+            host.engine(self.device)
+            if host.time_window is not None:  # (as above)
+                host.cover_window(self.device, np.zeros(1))
             if host.vector is not None:
                 *_, ei_k, _ = host.engine(self.device).sample_velocity(np.zeros(len(self)), d["z"], d["y"], d["x"], three_d=False,
                                                                         positions_are_f32=True, ei_hint=None, no_hint=True)  # fmt: skip
