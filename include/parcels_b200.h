@@ -438,6 +438,9 @@ enum pb_math_op {
     PB_MATH_BOX_MULLER_F32 = 5
 };
 int32_t pb_debug_math(pb_engine* e, int32_t op, int64_t n, const double* a, const double* b, double* out);
+/* The device cell table of axis `axis` (0 lon, 1 lat, 2 depth, 3 time) of a float64 rectilinear grid: `cells` records of 4 doubles
+ * {lo, hi, 1 / (hi - lo), 0} into `out`; `cells` must be the axis' node count - 1.  PB_ERR_INVALID when there is no such table. */
+int32_t pb_debug_axis_cells(pb_engine* e, int32_t axis, int64_t cells, double* out);
 
 /* ---- host-side passes of Kernel.execute / ParticleSet.execute over the particle columns, multi-threaded ----------------
  * The reference makes a few whole-column passes per call on the host: `pset._data["dt"][:] = dt` (_core/particleset.py:405,

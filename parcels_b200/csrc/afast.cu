@@ -55,24 +55,58 @@ cudaError_t launch_interleave(const float* u, const float* v, const float* w, lo
     return cudaGetLastError();
 }
 
+// per-axis cell tables (AxisCellRec, common.cuh): the side path's neighbour cell and reciprocal in one load
+__global__ void axis_cells_kernel(const double* __restrict__ a, int n, AxisCellRec* __restrict__ out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n - 1) return;
+    AxisCellRec c;
+    c.lo = a[i];
+    c.hi = a[i + 1];
+    c.rcp = 1.0 / (c.hi - c.lo);
+    c.pad_ = 0.0;
+    out[i] = c;
+}
+
+cudaError_t launch_axis_cells(const double* a, int n, AxisCellRec* out, cudaStream_t s) {
+    if (n < 2) return cudaSuccess;
+    axis_cells_kernel<<<(unsigned)((n - 1 + 255) / 256), 256, 0, s>>>(a, n, out);
+    return cudaGetLastError();
+}
+
 // ------------------------------------------------------------------------------------------------
 // axis search of the side path: the cell only (no bcoord division), neighbours of the cached cell first.
-// Same cell / sentinel as axis_search (common.cuh; reference _core/index_search.py:20-62).
+// Same cell / sentinel as axis_search (common.cuh; reference _core/index_search.py:20-62).  In two halves, so that the side path
+// has the loads of all four axes in flight before it tests any of them: axis_peek loads the cell record the neighbour test needs
+// (the neighbour on the side of x, or the cached cell itself) from the axis' cell table; axis_locate tests it and falls back to
+// the binary search.  `rcp` = 1 / (hi - lo) of the located cell (of the clipped cell for a sentinel), from the table.
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void axis_locate(const double* __restrict__ arr, int n, double x, AxisCell<double>& c) {
+// (n >= 2 on every axis the specialised kernel searches: agrid_fast_applies)
+struct CellPeek {
+    double lo, hi, rcp;
+};
+__device__ __forceinline__ CellPeek axis_peek(const AxisCellRec* __restrict__ tab, int n, double x, const AxisCell<double>& c) {
+    int j = c.idx;
+    if (c.idx >= 0) {
+        if (x > c.hi) j = c.idx + 1;
+        else if (x <= c.lo) j = c.idx - 1;
+    }
+    j = min(max(j, 0), n - 2);
+    const double2 b = ldg(reinterpret_cast<const double2*>(tab + j));
+    return CellPeek{b.x, b.y, ldg(&tab[j].rcp)};
+}
+__device__ __forceinline__ void axis_locate(const double* __restrict__ arr, const AxisCellRec* __restrict__ tab, int n, double x,
+                                            const CellPeek& nb, AxisCell<double>& c, double& rcp) {
     if (n < 2) {  // index_search.py:45-46
         c.idx = 0;
         return;
     }
     if (c.idx >= 0) {
         // lo < x <= hi of a cell inside the axis is exactly searchsorted(side="left") - 1 == that cell
-        if (x > c.lo && x <= c.hi) return;
+        if (x > c.lo && x <= c.hi) { rcp = nb.rcp; return; }
         if (x > c.hi && c.idx + 2 <= n - 1) {
-            const double nh = ldg(arr + c.idx + 2);
-            if (x <= nh) { c.lo = c.hi; c.hi = nh; c.idx += 1; return; }
+            if (x <= nb.hi) { c.lo = nb.lo; c.hi = nb.hi; c.idx += 1; rcp = nb.rcp; return; }
         } else if (x <= c.lo && c.idx >= 1) {
-            const double nl = ldg(arr + c.idx - 1);
-            if (x > nl) { c.hi = c.lo; c.lo = nl; c.idx -= 1; return; }
+            if (x > nb.lo) { c.lo = nb.lo; c.hi = nb.hi; c.idx -= 1; rcp = nb.rcp; return; }
         }
     }
     int l = 0, h = n;  // first i with arr[i] >= x   (side="left")
@@ -84,6 +118,7 @@ __device__ __forceinline__ void axis_locate(const double* __restrict__ arr, int 
     const int i = min(max(l - 1, 0), n - 2);
     c.lo = ldg(arr + i);
     c.hi = ldg(arr + i + 1);
+    rcp = ldg(&tab[i].rcp);
     c.idx = i;
     if (x < ldg(arr)) c.idx = -2;          // LEFT_OUT_OF_BOUNDS
     if (x > ldg(arr + n - 1)) c.idx = -1;  // RIGHT_OUT_OF_BOUNDS
@@ -126,6 +161,21 @@ __device__ __forceinline__ double2 lds_volatile(const double2* p) {
 #endif
 }
 
+// a 16-byte global -> shared copy that does not pass through registers (cp.async); this thread sees it after cp_async_wait
+__device__ __forceinline__ void cp_async16(float4* dst, const float4* src) {
+#ifdef PB_HOSTSIM
+    *dst = *src;
+#else
+    const unsigned a = (unsigned)__cvta_generic_to_shared(dst);
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" ::"r"(a), "l"(src) : "memory");
+#endif
+}
+__device__ __forceinline__ void cp_async_wait() {
+#ifndef PB_HOSTSIM
+    asm volatile("cp.async.wait_all;" ::: "memory");
+#endif
+}
+
 
 struct SideResult {
     double u, v, w;
@@ -133,6 +183,27 @@ struct SideResult {
     int flags;  // SIDE_*
 };
 enum { SIDE_FINAL = 1, SIDE_OUT_OF_TIME = 2, SIDE_REFILLED = 4, SIDE_SEARCHED = 8 };
+
+#ifdef PB_SIDE_PROFILE
+// Measurement build only (scripts/side_path_profile.py; the default build has none of this): clock64 counters of the evaluation's
+// phases, seen by the warp, summed over every warp of every launch since the last pb_side_profile_read.
+enum {
+    PROF_WARP_EVALS,        // warp-evaluations (one eval_fast call of a warp)
+    PROF_MISS_EVALS,        // ... of them with at least one lane in side_path
+    PROF_EVAL_CYCLES,       // cycles of all warp-evaluations
+    PROF_MISS_EVAL_CYCLES,  // ... of the ones with a miss
+    PROF_SIDE_CYCLES,       // cycles from the missing lanes' entry into side_path to their exit
+    PROF_SIDE_LANES,        // lane entries into side_path
+    PROF_N
+};
+__device__ unsigned long long pb_side_prof[PROF_N];
+extern "C" int pb_side_profile_read(unsigned long long* out) {  // copies the sums out and zeroes them; 0 on success
+    static const unsigned long long zero[PROF_N] = {};
+    if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpyFromSymbol(out, pb_side_prof, sizeof(zero)) != cudaSuccess) return 1;
+    return cudaMemcpyToSymbol(pb_side_prof, zero, sizeof(zero)) != cudaSuccess;
+}
+__device__ __forceinline__ bool prof_leader(unsigned mask) { return (int)(threadIdx.x & 31) == __ffs(mask) - 1; }
+#endif
 
 struct FastCtx {
     double lerp_t;  // sample time the T-lerped block in shared memory belongs to (-1: none)
@@ -143,6 +214,10 @@ struct FastCtx {
     bool searched;
     bool out_of_time;
     signed char len_t, len_z;  // (interface of the generic kernel skeleton; unused here)
+#ifdef PB_SIDE_PROFILE
+    bool prof_miss;  // this lane entered side_path in the current evaluation
+    unsigned long long prof[PROF_N];
+#endif
 };
 
 // NC: components sampled (2: fieldset.UV, 3: fieldset.UVW).  HZ: the grid has a depth axis with >= 2 levels.  SCHED: see the head
@@ -192,9 +267,16 @@ struct AFastPolicy {
         e.ei = ei;
         e.searched = false;
         e.len_t = e.len_z = -1;
+#ifdef PB_SIDE_PROFILE
+        for (int k = 0; k < PROF_N; ++k) e.prof[k] = 0;
+#endif
     }
     // ravel_index (basegrid.py:259-278) over the axes present of the last completed search; int64 arithmetic stored to int32
     __device__ static __forceinline__ void finish(Ctx& e, const AdvectParams& p) {
+#ifdef PB_SIDE_PROFILE
+        for (int k = 0; k < PROF_N; ++k)
+            if (e.prof[k]) atomicAdd(&pb_side_prof[k], e.prof[k]);
+#endif
         if (!e.searched) return;
         const int4 ix = *idx(e.raw);
         int gxi = ix.w;
@@ -204,7 +286,9 @@ struct AFastPolicy {
         e.ei = (int)r;
     }
 
-    // gather the (t, z, y, x) corner block of every component from the node-interleaved copy into this lane's raw columns
+    // gather the (t, z, y, x) corner block of every component from the node-interleaved copy into this lane's raw columns, with
+    // asynchronous copies: the raw block may only be read after cp_async_wait (the T-lerp, special_component), so the arithmetic
+    // in between runs under the DRAM latency
     __device__ static __forceinline__ void refill(const FieldDev& f, float4* raw, int ti, int zi, int yi, int xi) {
         const long long ot[2] = {wrap_idx(ti, f.T) * f.sT, up_idx(ti, f.T) * f.sT};
         const long long oz[2] = {wrap_idx(zi, f.Z) * f.sZ, up_idx(zi, f.Z) * f.sZ};
@@ -215,10 +299,10 @@ struct AFastPolicy {
         for (int pl = 0; pl < NV / 4; ++pl) {
             // records k = 4 pl .. 4 pl + 3,  k = (t * 2 + z) * 4 + y * 2 + x (HZ) | t * 4 + y * 2 + x: stored as they are loaded
             const long long o = ot[HZ ? (pl >> 1) : pl] + (HZ ? oz[pl & 1] : 0);
-            raw[(4 * pl + 0) * PB_FAST_BLOCK] = ldg(base + o + oy[0] + ox[0]);
-            raw[(4 * pl + 1) * PB_FAST_BLOCK] = ldg(base + o + oy[0] + ox[1]);
-            raw[(4 * pl + 2) * PB_FAST_BLOCK] = ldg(base + o + oy[1] + ox[0]);
-            raw[(4 * pl + 3) * PB_FAST_BLOCK] = ldg(base + o + oy[1] + ox[1]);
+            cp_async16(raw + (4 * pl + 0) * PB_FAST_BLOCK, base + o + oy[0] + ox[0]);
+            cp_async16(raw + (4 * pl + 1) * PB_FAST_BLOCK, base + o + oy[0] + ox[1]);
+            cp_async16(raw + (4 * pl + 2) * PB_FAST_BLOCK, base + o + oy[1] + ox[0]);
+            cp_async16(raw + (4 * pl + 3) * PB_FAST_BLOCK, base + o + oy[1] + ox[1]);
         }
     }
 
@@ -240,34 +324,31 @@ struct AFastPolicy {
         const double2 bz = HZ ? *cell(raw, 0) : double2{0.0, 0.0}, by = *cell(raw, 1), bx = *cell(raw, 2), bt = *cell(raw, 3);
         const int4 old = *idx(raw);  // key of the raw block: {ti, zi, yi, xi}
         AxisCell<double> ct{old.x, bt.x, bt.y}, cz{old.y, bz.x, bz.y}, cy{old.z, by.x, by.y}, cx{old.w, bx.x, bx.y};
-        const double wt = ct.hi - ct.lo, wz = cz.hi - cz.lo, wy = cy.hi - cy.lo, wx = cx.hi - cx.lo;  // (NaN for a poisoned cell)
         if (old.x >= 0 && !(ct.lo == ct.lo)) ct.idx = -100;  // (a poisoned cell is not a neighbour-search seed)
         if (old.y >= 0 && !(cz.lo == cz.lo)) cz.idx = -100;
         if (old.z >= 0 && !(cy.lo == cy.lo)) cy.idx = -100;
         if (old.w >= 0 && !(cx.lo == cx.lo)) cx.idx = -100;
-        axis_locate(g.time, g.nt, ts, ct);
+        const AxisCellRec* const* const tab = pp->cells;  // 0: lon, 1: lat, 2: depth, 3: time
+        const CellPeek pt = axis_peek(tab[3], g.nt, ts, ct), pz = HZ ? axis_peek(tab[2], g.nz, zs, cz) : CellPeek{0.0, 0.0, 0.0};
+        const CellPeek py = axis_peek(tab[1], g.ny, ys, cy), px = axis_peek(tab[0], g.nx, xs, cx);
+        double rt = 0.0, rz = 0.0, ry = 0.0, rx = 0.0;  // 1 / width of the located cells (the straight-line path's bcoord divisions)
+        axis_locate(g.time, tab[3], g.nt, ts, pt, ct, rt);
         const int ti = ct.idx;
         int zi = 0;
         if (HZ) {
-            axis_locate((const double*)g.depth, g.nz, zs, cz);
+            axis_locate((const double*)g.depth, tab[2], g.nz, zs, pz, cz, rz);
             zi = cz.idx;
         }
-        axis_locate((const double*)g.lat, g.ny, ys, cy);
-        axis_locate((const double*)g.lon, g.nx, xs, cx);
+        axis_locate((const double*)g.lat, tab[1], g.ny, ys, py, cy, ry);
+        axis_locate((const double*)g.lon, tab[0], g.nx, xs, px, cx, rx);
         const int yi = cy.idx, xi = cx.idx;
-        {   // cell widths changed: new reciprocals (the division itself: correctly rounded)
+        {
             double2* const rp = rcp(raw);
-            const double nwt = ct.hi - ct.lo, nwz = cz.hi - cz.lo, nwy = cy.hi - cy.lo, nwx = cx.hi - cx.lo;
-            if ((HZ && !(nwz == wz)) || !(nwy == wy)) {
-                double2 d;
-                d.x = 1.0 / nwz; d.y = 1.0 / nwy;
-                rp[0] = d;
-            }
-            if (!(nwx == wx) || !(nwt == wt)) {
-                double2 d;
-                d.x = 1.0 / nwx; d.y = 1.0 / nwt;
-                rp[PB_FAST_BLOCK] = d;
-            }
+            double2 d;
+            d.x = rz; d.y = ry;
+            rp[0] = d;
+            d.x = rx; d.y = rt;
+            rp[PB_FAST_BLOCK] = d;
         }
         int4 now;
         now.x = ti; now.y = zi; now.z = yi; now.w = xi;
@@ -303,6 +384,7 @@ struct AFastPolicy {
             const double eta = axis_bcoord(g.ny, ys, cy), xsi = axis_bcoord(g.nx, xs, cx);
             const bool two_t = tau > 0;             // lenT, per particle (float64 grid: no dtype depends on the batch)
             const bool two_z = HZ && !(zeta <= 0);  // lenZ, per particle (a NaN depth must poison the value)
+            cp_async_wait();
             double u = special_component<NV>(raw, 0, tau, zeta, eta, xsi, two_t, two_z);
             double v = special_component<NV>(raw, 1, tau, zeta, eta, xsi, two_t, two_z);
             double w = NC == 3 ? special_component<NV>(raw, 2, tau, zeta, eta, xsi, two_t, two_z) : 0.0;
@@ -335,6 +417,26 @@ struct AFastPolicy {
     template <int RENEW>
     __device__ static __forceinline__ void eval_fast(const AdvectParams& p, Ctx& e, const bool renew_rt, const bool first, const double ts,
                                                      const double zs, const double ys, const double xs, double& u, double& v, double& w) {
+#ifdef PB_SIDE_PROFILE
+        const unsigned am = __activemask();
+        e.prof_miss = false;
+        const long long c0 = clock64();
+        eval_body<RENEW>(p, e, renew_rt, first, ts, zs, ys, xs, u, v, w);
+        __syncwarp(am);
+        const long long dc = clock64() - c0;
+        const bool miss = __any_sync(am, e.prof_miss);
+        if (prof_leader(am)) {
+            e.prof[PROF_WARP_EVALS] += 1;
+            e.prof[PROF_EVAL_CYCLES] += dc;
+            if (miss) { e.prof[PROF_MISS_EVALS] += 1; e.prof[PROF_MISS_EVAL_CYCLES] += dc; }
+        }
+#else
+        eval_body<RENEW>(p, e, renew_rt, first, ts, zs, ys, xs, u, v, w);
+#endif
+    }
+    template <int RENEW>
+    __device__ static __forceinline__ void eval_body(const AdvectParams& p, Ctx& e, const bool renew_rt, const bool first, const double ts,
+                                                     const double zs, const double ys, const double xs, double& u, double& v, double& w) {
         const GridDev& g = p.g;
         const bool renew = RENEW < 0 ? renew_rt : (RENEW != 0);
         float4* const raw = e.raw;
@@ -353,7 +455,17 @@ struct AFastPolicy {
             hit = hit && (renew ? (ts > bt.x && ts <= bt.y) : (ts == e.lerp_t));
             if (hit || trip) break;
             SideResult r;
+#ifdef PB_SIDE_PROFILE
+            const unsigned sm = __activemask();
+            const long long s0 = clock64();
+#endif
             side_path(&p, raw, first ? 0 : 1, ts, zs, ys, xs, e.state, &r);
+#ifdef PB_SIDE_PROFILE
+            __syncwarp(sm);
+            if (prof_leader(sm)) e.prof[PROF_SIDE_CYCLES] += clock64() - s0;
+            e.prof[PROF_SIDE_LANES] += 1;
+            e.prof_miss = true;
+#endif
             e.state = r.state;
             if (r.flags & SIDE_OUT_OF_TIME) e.out_of_time = true;
             if (r.flags & SIDE_SEARCHED) e.searched = true;
@@ -382,6 +494,7 @@ struct AFastPolicy {
             // bilinear sum (:147-152) accumulated corner by corner in the reference's left-to-right order
             constexpr int NZ = HZ ? 2 : 1;
             const double wgt[4] = {w00, w01, w10, w11};
+            cp_async_wait();  // (the refill of a cell change in this evaluation)
 #pragma unroll
             for (int pr = 0; pr < 2; ++pr) {
                 double L[3][NZ][2];
@@ -448,7 +561,7 @@ struct AFastPolicy {
 // launch
 // ------------------------------------------------------------------------------------------------
 bool agrid_fast_applies(const AdvectParams& p, bool coord_f64, bool data_f64, bool has_time, int nc) {
-    if (!coord_f64 || data_f64 || !has_time || !p.f.il || p.f.windowed || p.g.curvilinear) return false;
+    if (!coord_f64 || data_f64 || !has_time || !p.f.il || !p.cells[0] || p.f.windowed || p.g.curvilinear) return false;
     if (!(p.scheme == PB_ADVECTION_RK4 || p.scheme == PB_ADVECTION_RK4_3D)) return false;
     if (nc == 3 && p.g.nz < 2) return false;
     return p.g.nt >= 2 && p.g.nx >= 2 && p.g.ny >= 2;

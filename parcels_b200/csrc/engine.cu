@@ -313,6 +313,9 @@ struct pb_engine {
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, tev0 = nullptr, tev1 = nullptr;
     // grid
     DevBuf lon, lat, depth, time, hkeys, hstarts, hcounts, hfaces, hbucket, cellproj, hqbox;
+    // float64 rectilinear grids: the cell tables of lon, lat, depth, time back to back (AxisCellRec); cellp[k] NULL: none
+    DevBuf cells;
+    const AxisCellRec* cellp[4] = {};
     int interp = 0;  // enum pb_interp
     GridDev g{};
     long long hash_nent = 0;  // entries of the resident spatial-hash table
@@ -464,7 +467,7 @@ void pb_engine_destroy(pb_engine* e) {
     for (DevBuf& b : e->fbuf) b.release();
     e->il.release();
     for (DevBuf* b : {&e->mdest, &e->mkeep, &e->mcount, &e->mbounds, &e->hqbox, &e->hbucket, &e->cellproj, &e->hkeys, &e->hstarts,
-                      &e->hcounts, &e->hfaces, &e->lon, &e->lat, &e->depth, &e->time, &e->snap, &e->sblock, &e->soffs, &e->sidx,
+                      &e->hcounts, &e->hfaces, &e->lon, &e->lat, &e->depth, &e->time, &e->cells, &e->snap, &e->sblock, &e->soffs, &e->sidx,
                       &e->sout, &e->samp_d, &e->samp_i, &e->ad_iters})
         b->release();
     for (int r = 0; r < PB_MIG_MAX_RANKS; ++r)
@@ -551,6 +554,31 @@ static int32_t upload_zt(pb_engine* e, const void* depth, int64_t nz, int32_t co
     return PB_OK;
 }
 
+// the cell tables of a float64 rectilinear grid (AxisCellRec), from the axes just uploaded
+static int32_t build_axis_cells(pb_engine* e) {
+    for (const AxisCellRec*& c : e->cellp) c = nullptr;
+    if (!e->coord_f64 || e->g.curvilinear) return PB_OK;
+    const GridDev& g = e->g;
+    const double* axes[4] = {(const double*)g.lon, (const double*)g.lat, (const double*)g.depth, g.time};
+    const int n[4] = {g.nx, g.ny, g.nz, g.nt};
+    size_t off[4], recs = 0;
+    for (int k = 0; k < 4; ++k) {
+        off[k] = recs;
+        if (axes[k] && n[k] >= 2) recs += (size_t)n[k] - 1;
+    }
+    if (!recs) return PB_OK;
+    int32_t rc = e->cells.ensure(recs * sizeof(AxisCellRec));
+    if (rc) return rc;
+    for (int k = 0; k < 4; ++k) {
+        if (!axes[k] || n[k] < 2) continue;
+        AxisCellRec* out = (AxisCellRec*)e->cells.p + off[k];
+        cudaError_t ce = launch_axis_cells(axes[k], n[k], out, e->stream);
+        if (ce != cudaSuccess) return fail(PB_ERR_CUDA, "axis_cells_kernel launch failed: %s", cudaGetErrorString(ce));
+        e->cellp[k] = out;
+    }
+    return PB_OK;
+}
+
 int32_t pb_grid_upload_rectilinear(pb_engine* e, const void* lon, int64_t nx, const void* lat, int64_t ny,
                                    const void* depth, int64_t nz, int32_t coord_is_f64, const double* time_s,
                                    int64_t nt, int32_t spherical, double deg2m, int64_t xdim_cells,
@@ -570,7 +598,8 @@ int32_t pb_grid_upload_rectilinear(pb_engine* e, const void* lon, int64_t nx, co
     e->g.curvilinear = 0;
     e->g.hkeys = nullptr; e->g.hstarts = nullptr; e->g.hcounts = nullptr; e->g.hfaces = nullptr; e->g.hnkeys = 0;
     e->g.hbucket = nullptr; e->g.cellproj = nullptr; e->g.hqbox = nullptr;
-    return upload_zt(e, depth, nz, coord_is_f64, time_s, nt, spherical, deg2m, xdim_cells, ydim_cells, zdim_cells);
+    if ((rc = upload_zt(e, depth, nz, coord_is_f64, time_s, nt, spherical, deg2m, xdim_cells, ydim_cells, zdim_cells))) return rc;
+    return build_axis_cells(e);
 }
 
 int32_t pb_grid_upload_curvilinear(pb_engine* e, const void* lon2d, const void* lat2d, int64_t ny, int64_t nx,
@@ -627,6 +656,7 @@ int32_t pb_grid_upload_curvilinear(pb_engine* e, const void* lon2d, const void* 
     e->hash_nent = n_entries;
     g.nx = (int)nx; g.ny = (int)ny;
     g.curvilinear = 1;
+    for (const AxisCellRec*& c : e->cellp) c = nullptr;  // (the tables of a rectilinear grid uploaded before)
     g.hash_bitwidth = hash_bitwidth;
     g.hkeys = (const unsigned int*)e->hkeys.p;
     g.hstarts = (const long long*)e->hstarts.p;
@@ -1059,6 +1089,7 @@ static void fill_advect_params(pb_engine* e, const Args* a, AdvectParams& p) {
     p.resume = a->resume; p.kernels_only = a->kernels_only;
     p.batch_levels = a->batch_levels;
     p.rep = e->d_rep;
+    for (int k = 0; k < 4; ++k) p.cells[k] = e->cellp[k];
 }
 }
 
@@ -1396,6 +1427,16 @@ int32_t pb_debug_normals(pb_engine* e, uint64_t seed, uint64_t rng_call, int64_t
     CK(cudaStreamSynchronize(e->stream));
     cudaFree(d_pid);
     cudaFree(d_out);
+    return PB_OK;
+}
+
+int32_t pb_debug_axis_cells(pb_engine* e, int32_t axis, int64_t cells, double* out) {
+    if (!e || !out || axis < 0 || axis > 3) return fail(PB_ERR_INVALID, "NULL argument or unknown axis");
+    const int n[4] = {e->g.nx, e->g.ny, e->g.nz, e->g.nt};
+    if (!e->cellp[axis] || cells != (int64_t)n[axis] - 1) return fail(PB_ERR_INVALID, "no cell table of %lld cells for axis %d", (long long)cells, axis);
+    CK(cudaSetDevice(e->device));
+    CK(cudaMemcpyAsync(out, e->cellp[axis], (size_t)cells * sizeof(AxisCellRec), cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
     return PB_OK;
 }
 

@@ -406,3 +406,12 @@ class Engine:
         out = np.empty((a.size, 2), dtype=np.float64)
         check(self._lib.pb_debug_math(self._h, self.MATH_OPS[op], a.size, ptr(a), ptr(b), ptr(out)))
         return out
+
+    AXES = {"lon": 0, "lat": 1, "depth": 2, "time": 3}
+
+    def debug_axis_cells(self, axis, nodes):
+        """The device cell table of a float64 rectilinear axis of `nodes` nodes: (nodes - 1, 4) float64 {lo, hi, 1 / (hi - lo), 0}
+        (see pb_debug_axis_cells)."""
+        out = np.empty((nodes - 1, 4), dtype=np.float64)
+        check(self._lib.pb_debug_axis_cells(self._h, self.AXES[axis], nodes - 1, ptr(out)))
+        return out
