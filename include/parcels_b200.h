@@ -309,6 +309,15 @@ typedef struct pb_rk45_args {
     int32_t batch_levels;       /* like the pb_advect_args field; the time bit applies to the first attempt of the first iteration */
 } pb_rk45_args;
 int32_t pb_advect_rk45(pb_engine* e, const pb_rk45_args* args, double* dt_inout, double* next_dt_inout, pb_report* rep);
+/* The same loop on the RESIDENT dt / next_dt / iteration columns of pb_particles_upload_resume (read them back with
+ * pb_particles_download_resume): the route of a domain-decomposed engine (mode D, below), where these travel with the particles,
+ * and the one RK45 entry point that runs there (rectilinear A-grid, XLinear_Velocity).  kernels_only must be 0.  A particle that
+ * leaves the owned slab stops mid-call with its dt, next_dt and iteration count, and the launch with resume = 1 on its new owner
+ * continues it.  Without waiting (pb_last_report collects the report); no batch-level clamp of the particles that left the loop
+ * early: pb_rk45_finalize_resident does it once the whole call is done, with the call's iteration count over all launches and
+ * ranks (the maximum of every pb_report.max_iters_done). */
+int32_t pb_advect_rk45_resident_async(pb_engine* e, const pb_rk45_args* args);
+int32_t pb_rk45_finalize_resident(pb_engine* e, double dt, double endtime, int64_t total_iters);
 
 /* ---- AdvectionDiffusionM1 / AdvectionDiffusionEM (kernels/_advectiondiffusion.py:21-117) under Kernel.execute's loop:
  * 2-D advection with fieldset.UV plus diffusion with the spatially varying diffusivity fields Kh_zonal / Kh_meridional
@@ -387,6 +396,19 @@ int32_t pb_decomp_set(pb_engine* e, int32_t nranks, int32_t rank, const double* 
 int32_t pb_migrate_count(pb_engine* e, int64_t* counts /* [nranks] records to send to each rank */);
 int32_t pb_migrate_pack(pb_engine* e, void* sendbuf_dev, int64_t capacity_records);
 int32_t pb_migrate_unpack(pb_engine* e, const void* recvbuf_dev, int64_t n_in);
+/* AdvectionRK45 (pb_advect_rk45_resident_async) and AdvectionDiffusionM1 / EM (pb_advect_diffusion) under mode D: a lane stopped
+ * mid-call continues on its new owner with its dt, next_dt and iteration count (M1 / EM: the count keys the Wiener increments,
+ * so the decomposed run draws the single-GPU run's increments).  pb_particles_upload_resume makes them resident columns (after
+ * pb_particles_upload, which drops them; NULL arrays upload zeros), and from then on every move of the set carries them:
+ * compaction, snapshot / restore, the in-kernel delivery (a 24-byte record per particle at the index of its 48-byte record, in
+ * the inbox after the record slots) and the collective exchange -- pb_migrate_pack_resume / pb_migrate_unpack_resume fill and
+ * read a second buffer of PB_MIGRATION_RESUME_BYTES per record, exchanged with the same counts as the records (the plain
+ * pack / unpack refuse an engine with resident resumable state). */
+#define PB_MIGRATION_RESUME_BYTES 24
+int32_t pb_particles_upload_resume(pb_engine* e, int64_t n, const double* dt, const double* next_dt, const int32_t* iters);
+int32_t pb_particles_download_resume(pb_engine* e, int64_t n, double* dt, double* next_dt, int32_t* iters);
+int32_t pb_migrate_pack_resume(pb_engine* e, void* sendbuf_dev, void* resume_sendbuf_dev, int64_t capacity_records);
+int32_t pb_migrate_unpack_resume(pb_engine* e, const void* recvbuf_dev, const void* resume_recvbuf_dev, int64_t n_in);
 
 /* In-kernel migration over peer memory (one box: NVLink / NVSwitch).  No reference counterpart.  Every rank owns an INBOX
  * (two slots of `capacity_records` 48-byte records + an arrival counter each) in its own HBM; its peers map it through CUDA IPC.

@@ -144,6 +144,12 @@ SYMBOLS = {
     "pb_advect_async": (C.c_int32, [_P, C.POINTER(AdvectArgs)]),
     "pb_advect_host": (C.c_int32, [_P, C.POINTER(AdvectArgs), C.c_int64, C.POINTER(ParticleArrays), C.c_int32, C.c_int32, C.POINTER(Report)]),
     "pb_advect_rk45": (C.c_int32, [_P, _P, _P, _P, _P]),
+    "pb_advect_rk45_resident_async": (C.c_int32, [_P, C.POINTER(Rk45Args)]),
+    "pb_rk45_finalize_resident": (C.c_int32, [_P, C.c_double, C.c_double, C.c_int64]),
+    "pb_particles_upload_resume": (C.c_int32, [_P, C.c_int64, _P, _P, _P]),
+    "pb_particles_download_resume": (C.c_int32, [_P, C.c_int64, _P, _P, _P]),
+    "pb_migrate_pack_resume": (C.c_int32, [_P, _P, _P, C.c_int64]),
+    "pb_migrate_unpack_resume": (C.c_int32, [_P, _P, _P, C.c_int64]),
     "pb_advect_diffusion": (C.c_int32, [_P, C.POINTER(AdvDiffArgs), C.POINTER(Report)]),
     "pb_advect_diffusion_async": (C.c_int32, [_P, C.POINTER(AdvDiffArgs)]),
     "pb_last_report": (C.c_int32, [_P, C.POINTER(Report)]),

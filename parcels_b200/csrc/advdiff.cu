@@ -57,7 +57,7 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, 2) advdiff_kernel(const AdvD
     unsigned long long my_steps = 0, my_refills = 0;
     int final_state = 0;
     long long my_iters = 0;
-    bool errored = false, deleted = false, oot = false, wait_window = false;
+    bool errored = false, deleted = false, oot = false, wait_window = false, migrate = false;
     long long err_iter = LLONG_MAX;
 
     if (i < p.P.n) {
@@ -96,6 +96,11 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, 2) advdiff_kernel(const AdvD
             if (p.max_iters >= 0 && it >= p.max_iters) break;
             const double tte = sign * (p.endtime - t);                                    // kernel.py:191
             if (!((state == PB_SUCCESS || state == PB_EVALUATE) && tte >= 0)) break;      // :193-195
+            // mode D: not ours (any more) -- before the window wait, as in advect_kernel
+            if (p.g.decomposed && !((double)x >= p.g.own_lo && (double)x < p.g.own_hi)) {
+                migrate = true;
+                break;
+            }
             const double dtp = (sign == 1) ? fmax(fmin(p.dt, tte), 0.0) : fmin(fmax(p.dt, -tte), 0.0);  // :199-203
             // every sample of M1 / EM is taken at the particle's own time (_advectiondiffusion.py:40-60,87-110): t must lie
             // within the resident time levels; outside the field's whole time interval is OutsideTimeInterval, not a wait
@@ -147,6 +152,9 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, 2) advdiff_kernel(const AdvD
             Val khm = evalK(q.fkm, z, y, x);
             if (q.spherical) khm = v_div_weak(khm, q.deg2m_sq);
             const Val by = v_sqrt(v_mul_weak(2.0, khm));
+            // mode D: a sample (UV, or Kh at x +- dres) left the owned + halo columns: the lane stops with state 99 before the
+            // delete handler below could turn it into a deletion
+            if (p.g.decomposed && state == 99) break;
 
             double sx, sy;  // the right-hand sides of `particles.dx += ...`, float64 (particles.dt is float64)
             if (q.em) {     // ax * dt + bx * dWx   (:85,101,115-117)
@@ -182,11 +190,18 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, 2) advdiff_kernel(const AdvD
         p.P.state[i] = state;
         p.P.ei[i] = ek.ei;
         if (q.iters) q.iters[i] = (int)it;
+        if (migrate && p.mig.on) {
+            MigRecord rec;
+            rec.t = t; rec.pid = pid;
+            rec.x = x; rec.y = y; rec.z = z; rec.dx = dx; rec.dy = dy; rec.dz = dz;
+            rec.state = state; rec.ei = ek.ei;
+            migrate = mig_deliver(p, i, rec, MigResume{0.0, 0.0, (int)it, 0});
+        }
     }
 
     const unsigned full = 0xffffffffu;
     unsigned long long s_steps = my_steps, s_ref = my_refills;
-    unsigned n_err = errored, n_del = deleted, n_oot = oot, n_ww = wait_window;
+    unsigned n_err = errored, n_del = deleted, n_oot = oot, n_ww = wait_window, n_mig = migrate;
     // with the delete handler an out-of-interval sample is not an error of the lane, but the host still needs the iteration
     // it happened in (the reference deletes the WHOLE evaluated view of that iteration, field.py:31-44)
     long long mx_it = my_iters, mn_err = (oot && deleted) ? my_iters - 1 : err_iter;
@@ -199,6 +214,7 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, 2) advdiff_kernel(const AdvD
         n_del += __shfl_xor_sync(full, n_del, o);
         n_oot += __shfl_xor_sync(full, n_oot, o);
         n_ww += __shfl_xor_sync(full, n_ww, o);
+        n_mig += __shfl_xor_sync(full, n_mig, o);
         mx_it = max(mx_it, __shfl_xor_sync(full, mx_it, o));
         mn_err = min(mn_err, __shfl_xor_sync(full, mn_err, o));
         mx_state = max(mx_state, __shfl_xor_sync(full, mx_state, o));
@@ -210,6 +226,7 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, 2) advdiff_kernel(const AdvD
         if (n_del) atomicAdd(&p.rep->n_deleted, (unsigned long long)n_del);
         if (n_oot) atomicAdd(&p.rep->n_out_of_time, (unsigned long long)n_oot);
         if (n_ww) atomicAdd(&p.rep->n_wait_window, (unsigned long long)n_ww);
+        if (n_mig) atomicAdd(&p.rep->n_migrate, (unsigned long long)n_mig);
         if (mx_it) atomicMax(&p.rep->max_iters_done, mx_it);
         if (mn_err != LLONG_MAX) atomicMin(&p.rep->first_error_iter, mn_err);
         if (mx_state) atomicMax(&p.rep->max_state, mx_state);

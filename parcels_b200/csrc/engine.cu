@@ -117,8 +117,9 @@ __global__ void mig_classify(ParticlesDev P, const double* __restrict__ bounds, 
     atomicAdd(&counts[d < 0 ? nranks : d], 1ULL);
 }
 
-__global__ void mig_pack(ParticlesDev P, const int* __restrict__ dest, int nranks, unsigned long long* cursors, MigRecord* send,
-                         long long* keep_idx) {
+// rsend (NULL: none) receives each leaver's resumable state R at the index of its record
+__global__ void mig_pack(ParticlesDev P, ResumeDev R, const int* __restrict__ dest, int nranks, unsigned long long* cursors,
+                         MigRecord* send, MigResume* rsend, long long* keep_idx) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= P.n) return;
     const int d = dest[i];
@@ -130,20 +131,26 @@ __global__ void mig_pack(ParticlesDev P, const int* __restrict__ dest, int nrank
         r.x = P.x[i]; r.y = P.y[i]; r.z = P.z[i];
         r.dx = P.dx[i]; r.dy = P.dy[i]; r.dz = P.dz[i];
         r.state = P.state[i]; r.ei = P.ei[i];
-        send[atomicAdd(&cursors[d], 1ULL)] = r;
+        const unsigned long long k = atomicAdd(&cursors[d], 1ULL);
+        send[k] = r;
+        if (rsend) rsend[k] = MigResume{R.dt[i], R.next_dt[i], R.iters[i], 0};
     }
 }
 
-__global__ void mig_compact(ParticlesDev src, ParticlesDev dst, const long long* __restrict__ keep_idx, long long n_keep) {
+// rs / rd: the resumable state, carried when rd.dt is not NULL
+__global__ void mig_compact(ParticlesDev src, ParticlesDev dst, ResumeDev rs, ResumeDev rd, const long long* __restrict__ keep_idx,
+                            long long n_keep) {
     const long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= n_keep) return;
     const long long i = keep_idx[k];
     dst.x[k] = src.x[i]; dst.y[k] = src.y[i]; dst.z[k] = src.z[i];
     dst.dx[k] = src.dx[i]; dst.dy[k] = src.dy[i]; dst.dz[k] = src.dz[i];
     dst.t[k] = src.t[i]; dst.state[k] = src.state[i]; dst.ei[k] = src.ei[i]; dst.pid[k] = src.pid[i];
+    if (rd.dt) { rd.dt[k] = rs.dt[i]; rd.next_dt[k] = rs.next_dt[i]; rd.iters[k] = rs.iters[i]; }
 }
 
-__global__ void mig_unpack(ParticlesDev dst, long long base, const MigRecord* __restrict__ recv, long long n_in) {
+__global__ void mig_unpack(ParticlesDev dst, ResumeDev rd, long long base, const MigRecord* __restrict__ recv,
+                           const MigResume* __restrict__ rrecv, long long n_in) {
     const long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= n_in) return;
     const MigRecord r = recv[k];
@@ -151,6 +158,10 @@ __global__ void mig_unpack(ParticlesDev dst, long long base, const MigRecord* __
     dst.x[j] = r.x; dst.y[j] = r.y; dst.z[j] = r.z;
     dst.dx[j] = r.dx; dst.dy[j] = r.dy; dst.dz[j] = r.dz;
     dst.t[j] = r.t; dst.state[j] = r.state; dst.ei[j] = r.ei; dst.pid[j] = r.pid;
+    if (rd.dt) {
+        const MigResume s = rrecv[k];
+        rd.dt[j] = s.dt; rd.next_dt[j] = s.next_dt; rd.iters[j] = s.iters;
+    }
 }
 
 
@@ -290,6 +301,17 @@ struct ParticleSoA {
         {8, false, true}};                                        // particle_id
     static_assert(offsetof(ParticlesDev, n) == NCOL * sizeof(void*), "one column per ParticlesDev pointer");
     DevBuf col[NCOL];
+    // each lane's resumable state (ResumeDev: dt, next_dt, iters), resident beside the columns above while pb_engine::resume_on;
+    // in the snapshot after them
+    static constexpr int NRES = 3;
+    static constexpr size_t res_es[NRES] = {8, 8, 4};
+    static constexpr size_t res_row_bytes = 20;
+    DevBuf res[NRES];
+    ResumeDev resume(long long lo = 0) const {
+        void* c[NRES];
+        for (int k = 0; k < NRES; ++k) c[k] = res[k].p ? (char*)res[k].p + (size_t)lo * res_es[k] : nullptr;
+        return ResumeDev{(double*)c[0], (double*)c[1], (int*)c[2]};
+    }
 
     // bytes per particle of the snapshot
     static constexpr size_t row_bytes(bool with_pid) {
@@ -347,6 +369,8 @@ struct pb_engine {
     DevBuf snap;  // snapshot of all particle arrays
     long long snap_n = -1;  // particle count the snapshot was taken at (-1: none); a new upload / compaction invalidates it
     bool snap_pid = false;  // the snapshot holds the particle ids too
+    bool resume_on = false;    // the resumable-state columns (ParticleSoA::res) are resident (pb_particles_upload_resume)
+    bool snap_resume = false;  // the snapshot holds them too
     // alternate SoA for compaction and migration (rebuild_resident); mode D (domain decomposition) migration work buffers
     ParticleSoA alt;
     DevBuf mdest, mkeep, mcount, mbounds;
@@ -462,8 +486,10 @@ void pb_engine_destroy(pb_engine* e) {
     if (!e) return;
     cudaSetDevice(e->device);
     cudaStreamSynchronize(e->stream);
-    for (ParticleSoA* s : {&e->cur, &e->alt})
+    for (ParticleSoA* s : {&e->cur, &e->alt}) {
         for (DevBuf& b : s->col) b.release();
+        for (DevBuf& b : s->res) b.release();
+    }
     for (DevBuf& b : e->fbuf) b.release();
     e->il.release();
     for (DevBuf* b : {&e->mdest, &e->mkeep, &e->mcount, &e->mbounds, &e->hqbox, &e->hbucket, &e->cellproj, &e->hkeys, &e->hstarts,
@@ -783,6 +809,37 @@ int32_t pb_particles_upload(pb_engine* e, int64_t n, const float* x, const float
     }
     e->n = n;
     e->snap_n = -1;
+    e->resume_on = false;  // (a new set: pb_particles_upload_resume gives it resumable state)
+    CK(cudaStreamSynchronize(e->stream));
+    return PB_OK;
+}
+
+int32_t pb_particles_upload_resume(pb_engine* e, int64_t n, const double* dt, const double* next_dt, const int32_t* iters) {
+    if (!e) return fail(PB_ERR_INVALID, "engine is NULL");
+    if (n != e->n) return fail(PB_ERR_INVALID, "resumable state of %lld particles but %lld are resident", (long long)n, (long long)e->n);
+    CK(cudaSetDevice(e->device));
+    const void* src[ParticleSoA::NRES] = {dt, next_dt, iters};
+    for (int k = 0; k < ParticleSoA::NRES; ++k) {
+        const size_t bytes = (size_t)n * ParticleSoA::res_es[k];
+        int32_t rc = e->cur.res[k].ensure(n ? bytes : 1);
+        if (rc) return rc;
+        if (!n) continue;
+        if (src[k]) CK(cudaMemcpyAsync(e->cur.res[k].p, src[k], bytes, cudaMemcpyHostToDevice, e->stream));
+        else CK(cudaMemsetAsync(e->cur.res[k].p, 0, bytes, e->stream));
+    }
+    CK(cudaStreamSynchronize(e->stream));
+    e->resume_on = true;
+    return PB_OK;
+}
+
+int32_t pb_particles_download_resume(pb_engine* e, int64_t n, double* dt, double* next_dt, int32_t* iters) {
+    if (!e) return fail(PB_ERR_INVALID, "engine is NULL");
+    if (!e->resume_on) return fail(PB_ERR_STATE, "no resumable state resident (pb_particles_upload_resume)");
+    if (n != e->n) return fail(PB_ERR_INVALID, "download of %lld particles but %lld are resident", (long long)n, (long long)e->n);
+    CK(cudaSetDevice(e->device));
+    void* dst[ParticleSoA::NRES] = {dt, next_dt, iters};
+    for (int k = 0; k < ParticleSoA::NRES; ++k)
+        if (dst[k] && n) CK(cudaMemcpyAsync(dst[k], e->cur.res[k].p, (size_t)n * ParticleSoA::res_es[k], cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));
     return PB_OK;
 }
@@ -817,7 +874,7 @@ int32_t pb_particles_snapshot(pb_engine* e) {
     if (!e) return fail(PB_ERR_INVALID, "engine is NULL");
     CK(cudaSetDevice(e->device));
     const size_t n = (size_t)e->n;
-    int32_t rc = e->snap.ensure(n ? n * ParticleSoA::row_bytes(true) : 1);
+    int32_t rc = e->snap.ensure(n ? n * (ParticleSoA::row_bytes(true) + (e->resume_on ? ParticleSoA::res_row_bytes : 0)) : 1);
     if (rc) return rc;
     size_t off = 0;
     for (int k = 0; k < ParticleSoA::NCOL; ++k) {
@@ -826,8 +883,13 @@ int32_t pb_particles_snapshot(pb_engine* e) {
         if (n) CK(cudaMemcpyAsync((char*)e->snap.p + off, e->cur.col[k].p, n * c.es, cudaMemcpyDeviceToDevice, e->stream));
         off += n * c.es;
     }
+    for (int k = 0; e->resume_on && k < ParticleSoA::NRES; ++k) {
+        if (n) CK(cudaMemcpyAsync((char*)e->snap.p + off, e->cur.res[k].p, n * ParticleSoA::res_es[k], cudaMemcpyDeviceToDevice, e->stream));
+        off += n * ParticleSoA::res_es[k];
+    }
     e->snap_n = (long long)n;
     e->snap_pid = e->have_pid;
+    e->snap_resume = e->resume_on;
     return PB_OK;
 }
 
@@ -837,7 +899,8 @@ int32_t pb_particles_restore(pb_engine* e) {
     PB_RANGE("pb_particles_restore");
     if (!e) return fail(PB_ERR_INVALID, "engine is NULL");
     CK(cudaSetDevice(e->device));
-    if (e->snap_n < 0 || e->snap.bytes < (size_t)e->snap_n * ParticleSoA::row_bytes(e->snap_pid))
+    if (e->snap_n < 0 ||
+        e->snap.bytes < (size_t)e->snap_n * (ParticleSoA::row_bytes(e->snap_pid) + (e->snap_resume ? ParticleSoA::res_row_bytes : 0)))
         return fail(PB_ERR_STATE, "no snapshot of the resident set to restore (the set was replaced or compacted since pb_particles_snapshot)");
     const size_t n = (size_t)e->snap_n;  // (stream-ordered after a pending advect launch: restore + launch sequences need no host sync)
     if (e->snap_n != e->n && !e->snap_pid)
@@ -852,6 +915,14 @@ int32_t pb_particles_restore(pb_engine* e) {
         if (n) CK(cudaMemcpyAsync(b.p, (char*)e->snap.p + off, n * c.es, cudaMemcpyDeviceToDevice, e->stream));
         off += n * c.es;
     }
+    for (int k = 0; e->snap_resume && k < ParticleSoA::NRES; ++k) {
+        DevBuf& b = e->cur.res[k];
+        int32_t rc = b.ensure(n ? n * ParticleSoA::res_es[k] : 1);
+        if (rc) return rc;
+        if (n) CK(cudaMemcpyAsync(b.p, (char*)e->snap.p + off, n * ParticleSoA::res_es[k], cudaMemcpyDeviceToDevice, e->stream));
+        off += n * ParticleSoA::res_es[k];
+    }
+    e->resume_on = e->snap_resume;
     if (e->snap_pid) e->have_pid = true;
     e->n = (long long)n;
     return PB_OK;
@@ -1093,6 +1164,20 @@ static void fill_advect_params(pb_engine* e, const Args* a, AdvectParams& p) {
 }
 }
 
+// in-kernel migration (connected over peer memory, mode D): where the kernels deliver a leaving particle
+static int32_t fill_mig(pb_engine* e, AdvectParams& p) {
+    if (e->mig_on && e->g.decomposed) {
+        if (!e->have_pid) return fail(PB_ERR_STATE, "migration needs particle_id");
+        for (int r = 0; r < e->nranks; ++r) p.mig.peer[r] = e->mig_peer[r];
+        p.mig.bounds = (const double*)e->mbounds.p;
+        p.mig.cap = e->mig_cap;
+        p.mig.nranks = e->nranks; p.mig.rank = e->rank;
+        p.mig.slot = e->mig_slot;
+        p.mig.on = 1;
+    }
+    return PB_OK;
+}
+
 // validation + kernel parameters shared by pb_advect_async and pb_advect_host (pb_advect_host sets p.P per chunk)
 static int32_t prepare_advect(pb_engine* e, const pb_advect_args* a, AdvectParams& p, int& nc) {
     if (!e || !a) return fail(PB_ERR_INVALID, "NULL argument");
@@ -1111,16 +1196,7 @@ static int32_t prepare_advect(pb_engine* e, const pb_advect_args* a, AdvectParam
     p.kh_zonal = a->kh_zonal; p.kh_meridional = a->kh_meridional; p.kh_deg2m = a->kh_deg2m;
     p.seed = a->seed; p.rng_call = a->rng_call;
     p.hint_all_zero = a->hint_all_zero;
-    if (e->mig_on && e->g.decomposed) {
-        if (!e->have_pid) return fail(PB_ERR_STATE, "migration needs particle_id");
-        for (int r = 0; r < e->nranks; ++r) p.mig.peer[r] = e->mig_peer[r];
-        p.mig.bounds = (const double*)e->mbounds.p;
-        p.mig.cap = e->mig_cap;
-        p.mig.nranks = e->nranks; p.mig.rank = e->rank;
-        p.mig.slot = e->mig_slot;
-        p.mig.on = 1;
-    }
-    return PB_OK;
+    return fill_mig(e, p);
 }
 
 static cudaError_t launch_advect_kernel(pb_engine* e, const AdvectParams& p, int nc, cudaStream_t stream) {
@@ -1188,6 +1264,7 @@ int32_t pb_advect_host(pb_engine* e, const pb_advect_args* a, int64_t n, const p
     if ((rc = e->snap.ensure(n ? (size_t)n * ParticleSoA::row_bytes(true) : 1))) return rc;
     e->have_pid = h->particle_id != nullptr;
     e->snap_pid = e->have_pid;
+    e->resume_on = e->snap_resume = false;
     e->n = n;
     e->snap_n = n;  // the chunks below write the start-of-interval copy
     p.lone_particle = n == 1;
@@ -1341,6 +1418,46 @@ int32_t pb_advect_rk45(pb_engine* e, const pb_rk45_args* a, double* dt_inout, do
     return PB_OK;
 }
 
+// AdvectionRK45 on the RESIDENT dt / next_dt / iteration columns (pb_particles_upload_resume): the route of a domain-decomposed
+// engine, where these travel with the particles.  No finalize clamp: pb_rk45_finalize_resident once the whole call is done.
+int32_t pb_advect_rk45_resident_async(pb_engine* e, const pb_rk45_args* a) {
+    PB_RANGE("pb_advect_rk45_resident");
+    if (!e || !a) return fail(PB_ERR_INVALID, "NULL argument");
+    if (a->dt == 0.0 || a->dt != a->dt) return fail(PB_ERR_INVALID, "dt must be a non-zero number");
+    if (a->kernels_only) return fail(PB_ERR_INVALID, "pb_advect_rk45_resident runs whole loop iterations (kernels_only = 0)");
+    if (!e->resume_on) return fail(PB_ERR_STATE, "dt / next_dt / iteration columns not resident (pb_particles_upload_resume)");
+    int32_t rc = check_fields(e, 2);
+    if (rc) return rc;
+    if (e->interp != PB_INTERP_XLINEAR_VELOCITY || e->g.curvilinear)
+        return fail(PB_ERR_INVALID, "pb_advect_rk45_resident runs on rectilinear A-grids with XLinear_Velocity");
+    CK(cudaSetDevice(e->device));
+    AdvectParams p{};
+    fill_advect_params(e, a, p);
+    p.scheme = PB_ADVECTION_RK45;
+    p.lone_particle = e->n == 1;
+    if ((rc = fill_mig(e, p))) return rc;
+    if ((rc = begin_launch(e))) return rc;
+    if (e->n > 0) {
+        const ResumeDev r = e->cur.resume();
+        cudaError_t ce = launch_rk45(p, r.dt, r.next_dt, r.iters, a->next_dt_is_f32, a->tol, a->min_dt, a->max_dt, e->coord_f64 != 0,
+                                     e->f_f64[0] != 0, e->g.nt > 0, e->stream);
+        if (ce != cudaSuccess) return fail(PB_ERR_CUDA, "rk45_kernel launch failed: %s", cudaGetErrorString(ce));
+    }
+    return end_launch(e);
+}
+
+int32_t pb_rk45_finalize_resident(pb_engine* e, double dt, double endtime, int64_t total_iters) {
+    if (!e) return fail(PB_ERR_INVALID, "engine is NULL");
+    if (!e->resume_on) return fail(PB_ERR_STATE, "dt / next_dt / iteration columns not resident (pb_particles_upload_resume)");
+    if (e->pending) return fail(PB_ERR_STATE, "an advect call is pending: call pb_last_report first");
+    CK(cudaSetDevice(e->device));
+    const ResumeDev r = e->cur.resume();
+    cudaError_t ce = launch_rk45_finalize(e->cur.view(e->n), r.dt, r.iters, total_iters, endtime, dt > 0 ? 1 : -1, e->stream);
+    if (ce != cudaSuccess) return fail(PB_ERR_CUDA, "rk45_finalize launch failed: %s", cudaGetErrorString(ce));
+    CK(cudaStreamSynchronize(e->stream));
+    return PB_OK;
+}
+
 // FieldDev of a scalar field slot (slots 3.. hold the scalar fields)
 static int32_t scalar_field_desc(pb_engine* e, int32_t slot, FieldDev& f) {
     if (slot < 3 || slot >= PB_MAX_FIELDS || !e->fptr[slot]) return fail(PB_ERR_STATE, "no scalar field in slot %d", slot);
@@ -1355,9 +1472,12 @@ int32_t pb_advect_diffusion_async(pb_engine* e, const pb_advdiff_args* a) {
     if (!(a->dres == a->dres) || a->dres == 0.0) return fail(PB_ERR_INVALID, "dres must be a non-zero number");
     int32_t rc = check_fields(e, 2);
     if (rc) return rc;
-    if ((e->interp != PB_INTERP_XLINEAR_VELOCITY && e->interp != PB_INTERP_CGRID_VELOCITY) || e->g.curvilinear || e->g.decomposed)
-        return fail(PB_ERR_INVALID, "AdvectionDiffusionM1/EM run on rectilinear fields with XLinear_Velocity or CGrid_Velocity, "
-                                    "not under domain decomposition");
+    if ((e->interp != PB_INTERP_XLINEAR_VELOCITY && e->interp != PB_INTERP_CGRID_VELOCITY) || e->g.curvilinear)
+        return fail(PB_ERR_INVALID, "AdvectionDiffusionM1/EM run on rectilinear fields with XLinear_Velocity or CGrid_Velocity");
+    // under domain decomposition every lane's iteration count travels with its particle: a resident column
+    if (e->g.decomposed && (e->interp != PB_INTERP_XLINEAR_VELOCITY || !e->resume_on))
+        return fail(PB_ERR_INVALID, "AdvectionDiffusionM1/EM under domain decomposition run with XLinear_Velocity on the resident "
+                                    "iteration columns (pb_particles_upload_resume)");
     if (!e->have_pid) return fail(PB_ERR_STATE, "diffusion needs particle_id (RNG counter)");
     FieldDev fkz, fkm;
     if ((rc = scalar_field_desc(e, a->kh_zonal_slot, fkz))) return rc;
@@ -1371,9 +1491,13 @@ int32_t pb_advect_diffusion_async(pb_engine* e, const pb_advdiff_args* a) {
     AdvectParams p{};
     fill_advect_params(e, a, p);
     p.seed = a->seed; p.rng_call = a->rng_call;
-    // time-windowed fields: the lanes' iteration counts survive into the resumed launches (resident fields need none)
+    if ((rc = fill_mig(e, p))) return rc;
+    // time-windowed fields: the lanes' iteration counts survive into the resumed launches (resident fields need none); with the
+    // resumable-state columns resident (mode D) they live there
     int* iters = nullptr;
-    if (e->ring) {
+    if (e->resume_on) {
+        iters = e->cur.resume().iters;
+    } else if (e->ring) {
         if ((rc = e->ad_iters.ensure(e->n ? (size_t)e->n * sizeof(int) : 1))) return rc;
         iters = (int*)e->ad_iters.p;
     }
@@ -1562,8 +1686,9 @@ int32_t pb_output_gather(pb_engine* e, int64_t n_selected, int64_t* index, float
 
 // The new resident set, built in the alternate columns: the current rows keep_idx[0..n_keep), then n_in arrival records; the
 // alternates then become current.  headroom: allocate 25 % more than needed (fewer reallocations when the count drifts).
-static int32_t rebuild_resident(pb_engine* e, const long long* keep_idx, long long n_keep, const MigRecord* arrivals, long long n_in,
-                                bool headroom) {
+// With the resumable-state columns resident they are carried too (arrivals_resume: the arrivals' MigResume at the same index).
+static int32_t rebuild_resident(pb_engine* e, const long long* keep_idx, long long n_keep, const MigRecord* arrivals,
+                                const MigResume* arrivals_resume, long long n_in, bool headroom) {
     const long long n_new = n_keep + n_in;
     const size_t cap = n_new ? (size_t)n_new : 1;
     for (int k = 0; k < ParticleSoA::NCOL; ++k) {
@@ -1571,13 +1696,20 @@ static int32_t rebuild_resident(pb_engine* e, const long long* keep_idx, long lo
         int32_t rc = e->alt.col[k].ensure(headroom ? bytes + bytes / 4 : bytes);
         if (rc) return rc;
     }
+    for (int k = 0; e->resume_on && k < ParticleSoA::NRES; ++k) {
+        const size_t bytes = cap * ParticleSoA::res_es[k];
+        int32_t rc = e->alt.res[k].ensure(headroom ? bytes + bytes / 4 : bytes);
+        if (rc) return rc;
+    }
+    if (e->resume_on && n_in > 0 && !arrivals_resume) return fail(PB_ERR_INVALID, "arrivals without their resumable state");
     const ParticlesDev dst = e->alt.view(n_new);
+    const ResumeDev rsrc = e->resume_on ? e->cur.resume() : ResumeDev{}, rdst = e->resume_on ? e->alt.resume() : ResumeDev{};
     if (n_keep > 0) {
-        mig_compact<<<(unsigned)((n_keep + 255) / 256), 256, 0, e->stream>>>(e->cur.view(e->n), dst, keep_idx, n_keep);
+        mig_compact<<<(unsigned)((n_keep + 255) / 256), 256, 0, e->stream>>>(e->cur.view(e->n), dst, rsrc, rdst, keep_idx, n_keep);
         CK(cudaGetLastError());
     }
     if (n_in > 0) {
-        mig_unpack<<<(unsigned)((n_in + 255) / 256), 256, 0, e->stream>>>(dst, n_keep, arrivals, n_in);
+        mig_unpack<<<(unsigned)((n_in + 255) / 256), 256, 0, e->stream>>>(dst, rdst, n_keep, arrivals, arrivals_resume, n_in);
         CK(cudaGetLastError());
     }
     CK(cudaStreamSynchronize(e->stream));
@@ -1598,7 +1730,7 @@ int32_t pb_particles_remove_deleted(pb_engine* e, int64_t* n_left) {
     if (rc) return rc;
     e->n_selected = -1;
     if (keep == e->n) { *n_left = keep; return PB_OK; }
-    if ((rc = rebuild_resident(e, (const long long*)e->sidx.p, keep, nullptr, 0, false))) return rc;
+    if ((rc = rebuild_resident(e, (const long long*)e->sidx.p, keep, nullptr, nullptr, 0, false))) return rc;
     *n_left = keep;
     return PB_OK;
 }
@@ -1628,11 +1760,9 @@ int32_t pb_migrate_count(pb_engine* e, int64_t* counts) {
     return PB_OK;
 }
 
-int32_t pb_migrate_pack(pb_engine* e, void* sendbuf_dev, int64_t capacity_records) {
-    PB_RANGE("pb_migrate_pack");
-    if (!e) return fail(PB_ERR_INVALID, "engine is NULL");
+static int32_t migrate_pack(pb_engine* e, void* sendbuf_dev, void* resume_sendbuf_dev, int64_t capacity_records) {
     if (e->n_send > capacity_records) return fail(PB_ERR_INVALID, "send buffer holds %lld records, %lld needed", (long long)capacity_records, e->n_send);
-    if (e->n_send && !sendbuf_dev) return fail(PB_ERR_INVALID, "NULL send buffer");
+    if (e->n_send && (!sendbuf_dev || (e->resume_on && !resume_sendbuf_dev))) return fail(PB_ERR_INVALID, "NULL send buffer");
     CK(cudaSetDevice(e->device));
     const int nr = e->nranks;
     // cursors: [0..nr-1] = exclusive prefix of the per-destination counts, [nr] = 0 (keep cursor)
@@ -1642,20 +1772,47 @@ int32_t pb_migrate_pack(pb_engine* e, void* sendbuf_dev, int64_t capacity_record
     int32_t rc;
     if ((rc = e->mkeep.ensure(e->n_keep ? e->n_keep * 8 : 8))) return rc;
     if (e->n > 0) {
-        mig_pack<<<(unsigned)((e->n + 255) / 256), 256, 0, e->stream>>>(e->cur.view(e->n), (const int*)e->mdest.p, nr,
-                                                                        (unsigned long long*)e->mcount.p, (MigRecord*)sendbuf_dev,
-                                                                        (long long*)e->mkeep.p);
+        mig_pack<<<(unsigned)((e->n + 255) / 256), 256, 0, e->stream>>>(
+            e->cur.view(e->n), e->resume_on ? e->cur.resume() : ResumeDev{}, (const int*)e->mdest.p, nr, (unsigned long long*)e->mcount.p,
+            (MigRecord*)sendbuf_dev, e->resume_on ? (MigResume*)resume_sendbuf_dev : nullptr, (long long*)e->mkeep.p);
         CK(cudaGetLastError());
     }
     CK(cudaStreamSynchronize(e->stream));  // cur goes out of scope; the caller hands sendbuf to NCCL next
     return PB_OK;
 }
 
+int32_t pb_migrate_pack(pb_engine* e, void* sendbuf_dev, int64_t capacity_records) {
+    PB_RANGE("pb_migrate_pack");
+    if (!e) return fail(PB_ERR_INVALID, "engine is NULL");
+    if (e->resume_on) return fail(PB_ERR_STATE, "resumable state resident: pb_migrate_pack_resume carries it");
+    return migrate_pack(e, sendbuf_dev, nullptr, capacity_records);
+}
+
+int32_t pb_migrate_pack_resume(pb_engine* e, void* sendbuf_dev, void* resume_sendbuf_dev, int64_t capacity_records) {
+    PB_RANGE("pb_migrate_pack_resume");
+    if (!e) return fail(PB_ERR_INVALID, "engine is NULL");
+    if (!e->resume_on) return fail(PB_ERR_STATE, "no resumable state resident (pb_particles_upload_resume)");
+    return migrate_pack(e, sendbuf_dev, resume_sendbuf_dev, capacity_records);
+}
+
 int32_t pb_migrate_unpack(pb_engine* e, const void* recvbuf_dev, int64_t n_in) {
     PB_RANGE("pb_migrate_unpack");
     if (!e || n_in < 0 || (n_in && !recvbuf_dev)) return fail(PB_ERR_INVALID, "bad argument");
+    if (e->resume_on) return fail(PB_ERR_STATE, "resumable state resident: pb_migrate_unpack_resume carries it");
     CK(cudaSetDevice(e->device));
-    int32_t rc = rebuild_resident(e, (const long long*)e->mkeep.p, e->n_keep, (const MigRecord*)recvbuf_dev, n_in, true);
+    int32_t rc = rebuild_resident(e, (const long long*)e->mkeep.p, e->n_keep, (const MigRecord*)recvbuf_dev, nullptr, n_in, true);
+    if (rc) return rc;
+    e->n_send = 0;
+    return PB_OK;
+}
+
+int32_t pb_migrate_unpack_resume(pb_engine* e, const void* recvbuf_dev, const void* resume_recvbuf_dev, int64_t n_in) {
+    PB_RANGE("pb_migrate_unpack_resume");
+    if (!e || n_in < 0 || (n_in && (!recvbuf_dev || !resume_recvbuf_dev))) return fail(PB_ERR_INVALID, "bad argument");
+    if (!e->resume_on) return fail(PB_ERR_STATE, "no resumable state resident (pb_particles_upload_resume)");
+    CK(cudaSetDevice(e->device));
+    int32_t rc = rebuild_resident(e, (const long long*)e->mkeep.p, e->n_keep, (const MigRecord*)recvbuf_dev,
+                                  (const MigResume*)resume_recvbuf_dev, n_in, true);
     if (rc) return rc;
     e->n_send = 0;
     return PB_OK;
@@ -1672,7 +1829,8 @@ int32_t pb_migrate_p2p_init(pb_engine* e, int64_t capacity_records, uint8_t* ipc
     if (e->nranks > PB_MIG_MAX_RANKS) return fail(PB_ERR_INVALID, "in-kernel migration supports <= %d ranks", PB_MIG_MAX_RANKS);
     if (e->mig_base) return fail(PB_ERR_STATE, "pb_migrate_p2p_init called twice");
     CK(cudaSetDevice(e->device));
-    const size_t bytes = 2 * (size_t)PB_MIG_HEADER_BYTES + 2 * (size_t)capacity_records * sizeof(MigRecord);
+    // [header 0][header 1][records of slot 0][records of slot 1][MigResume of slot 0][MigResume of slot 1] (common.cuh)
+    const size_t bytes = 2 * (size_t)PB_MIG_HEADER_BYTES + 2 * (size_t)capacity_records * (sizeof(MigRecord) + sizeof(MigResume));
     void* p = nullptr;
     CK(cudaMalloc(&p, bytes));  // (its own allocation: IPC handles export whole allocations)
     e->mig_base = (unsigned char*)p;
@@ -1736,7 +1894,9 @@ int32_t pb_migrate_p2p_finish(pb_engine* e, int64_t* n_in_out, int64_t* n_now) {
     const unsigned long long arrived = *e->h_mig_count;
     const long long n_in = (long long)(arrived < (unsigned long long)e->mig_cap ? arrived : (unsigned long long)e->mig_cap);
     if (keep != e->n || n_in > 0)
-        if ((rc = rebuild_resident(e, (const long long*)e->sidx.p, keep, mig_records(e->mig_base, slot, e->mig_cap), n_in, true))) return rc;
+        if ((rc = rebuild_resident(e, (const long long*)e->sidx.p, keep, mig_records(e->mig_base, slot, e->mig_cap),
+                                   mig_resume(e->mig_base, slot, e->mig_cap), n_in, true)))
+            return rc;
     // this slot is written again two rounds from now, after at least one more barrier: reset its counter now
     CK(cudaMemsetAsync(mig_counter(e->mig_base, slot), 0, 8, e->stream));
     e->mig_slot ^= 1;

@@ -22,7 +22,7 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, PB_MINBLOCKS) rk45_kernel(co
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     unsigned long long my_steps = 0, my_evals = 0;
     long long my_iters = 0;
-    bool stalled = false, wait_window = false;
+    bool stalled = false, wait_window = false, migrate = false, halo = false;
     int final_state = 0;
     if (i < p.P.n) {
         // Butcher tableau of _advection.py:96-106, the same Python float expressions
@@ -56,6 +56,12 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, PB_MINBLOCKS) rk45_kernel(co
             if (p.max_iters >= 0 && it >= p.max_iters) break;
             const double tte = sign * (p.endtime - t);
             if (!((e.state == PB_SUCCESS || e.state == PB_EVALUATE) && tte >= 0)) break;
+            // mode D: not ours (any more).  Tested before the window wait, as in advect_kernel: the new owner, whose window slides in
+            // lock-step with this one, makes the same wait decision
+            if (p.g.decomposed && !((double)x >= p.g.own_lo && (double)x < p.g.own_hi)) {
+                migrate = true;
+                break;
+            }
             dt = (sign == 1) ? fmax(fmin(dt, tte), 0.0) : fmin(fmax(dt, -tte), 0.0);  // kernel.py:199-203
             if (dt == 0.0 && tte > 0) {  // the reference never terminates here (t cannot advance): report instead of spinning
                 stalled = true;
@@ -116,6 +122,12 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, PB_MINBLOCKS) rk45_kernel(co
                 }
                 }
                 my_evals += 6;
+                // mode D: a stage position left the owned + halo columns (state 99, which the line `e.state = good ? ...` below
+                // would overwrite): the lane stops with it
+                if (p.g.decomposed && e.state == 99) {
+                    halo = true;
+                    break;
+                }
                 double x4 = mulc(u[0], b4[0]), y4 = mulc(v[0], b4[0]), x5 = mulc(u[0], b5[0]), y5 = mulc(v[0], b5[0]);
                 for (int j = 1; j < 5; ++j) {
                     x4 = x4 + u[j].v * b4[j];
@@ -144,6 +156,7 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, PB_MINBLOCKS) rk45_kernel(co
                 // clamped dt is below min_dt still advances t by min_dt in the position update
                 if (fabs(dt) < fabs(q.min_dt)) dt = q.min_dt * sgn_dt;
             } while (e.state == PB_REPEAT);
+            if (halo) break;
             if (p.kernels_only) { ++it; break; }  // mixed lists: the host finishes the iteration (stepwise.py)
             if (p.delete_on_error && e.state >= 50) e.state = PB_DELETE;  // never true after RK45 (see the header comment)
             if (e.state == PB_EVALUATE || e.state == PB_SUCCESS) {
@@ -165,10 +178,17 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, PB_MINBLOCKS) rk45_kernel(co
         q.dt[i] = dt;
         q.next_dt[i] = ndt;
         q.iters[i] = (int)it;
+        if (migrate && p.mig.on) {
+            MigRecord rec;
+            rec.t = t; rec.pid = p.P.pid[i];
+            rec.x = x; rec.y = y; rec.z = z; rec.dx = dx; rec.dy = dy; rec.dz = dz;
+            rec.state = final_state; rec.ei = e.ei;
+            migrate = mig_deliver(p, i, rec, MigResume{dt, ndt, (int)it, 0});
+        }
     }
     const unsigned full = 0xffffffffu;
     unsigned long long s_steps = my_steps, s_ev = my_evals;
-    unsigned n_stall = stalled, n_ww = wait_window;
+    unsigned n_stall = stalled, n_ww = wait_window, n_mig = migrate;
     long long mx_it = my_iters;
     int mx_state = final_state;
 #pragma unroll
@@ -177,6 +197,7 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, PB_MINBLOCKS) rk45_kernel(co
         s_ev += __shfl_xor_sync(full, s_ev, o);
         n_stall += __shfl_xor_sync(full, n_stall, o);
         n_ww += __shfl_xor_sync(full, n_ww, o);
+        n_mig += __shfl_xor_sync(full, n_mig, o);
         mx_it = max(mx_it, __shfl_xor_sync(full, mx_it, o));
         mx_state = max(mx_state, __shfl_xor_sync(full, mx_state, o));
     }
@@ -185,6 +206,7 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, PB_MINBLOCKS) rk45_kernel(co
         if (s_ev) atomicAdd(&p.rep->cache_refills, s_ev);  // RK45: the number of field evaluations (6 per attempt)
         if (n_stall) atomicAdd(&p.rep->n_error, (unsigned long long)n_stall);
         if (n_ww) atomicAdd(&p.rep->n_wait_window, (unsigned long long)n_ww);
+        if (n_mig) atomicAdd(&p.rep->n_migrate, (unsigned long long)n_mig);
         if (mx_it) atomicMax(&p.rep->max_iters_done, mx_it);
         if (mx_state) atomicMax(&p.rep->max_state, mx_state);
     }

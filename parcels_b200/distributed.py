@@ -79,6 +79,7 @@ def allreduce_sum(value: float, dist, device="cpu") -> float:
 # mode D
 # --------------------------------------------------------------------------------------------------
 RECORD_BYTES = 48  # PB_MIGRATION_RECORD_BYTES
+RESUME_BYTES = 24  # PB_MIGRATION_RESUME_BYTES
 
 
 def slab_plan(lon, world: int, halo_cells: int) -> list[dict]:
@@ -146,6 +147,17 @@ class DecomposedFieldSet:
                                        xdim=np.asarray(lon).size - 1)  # fmt: skip  (GLOBAL cell count: ei stays global)
         self._attach()
 
+    def add_field(self, name, data, interp_method="linear", time_window=None):
+        """``FieldSet.add_field`` of a GLOBAL (T, Z, Y, X) field on the velocity grid (e.g. Kh_zonal / Kh_meridional of
+        AdvectionDiffusionM1 / EM), cut to this rank's columns -- one time level at a time when it streams (``time_window``)."""
+        sl = slice(self.plan["lo"], self.plan["hi"] + 1)
+        slab = np.ascontiguousarray(np.asarray(data)[..., sl]) if time_window is None else _SlabLevels(data, sl)
+        return self.fs.add_field(name, slab, interp_method=interp_method, time_window=time_window)
+
+    def add_context(self, name, value):
+        """``FieldSet.add_context`` (``dres``, ``RK45_tol``, ``RK45_min_dt``, ``RK45_max_dt``, ...)."""
+        self.fs.add_context(name, value)
+
     @classmethod
     def from_slab(cls, fs, plan, *, rank, world, device):
         """Wrap a FieldSet that already holds ONLY this rank's slab (built with the GLOBAL ``xdim``), e.g. when
@@ -176,10 +188,11 @@ def _sync(device):
         torch.cuda.synchronize(device)
 
 
-def _exchange(eng, counts, dist, device):
+def _exchange(eng, counts, dist, device, resume=False):
     """One migration round: every rank's per-destination counts -> ONE all-gather (each rank then knows what it sends, what it
     receives and whether anybody moves at all) -> records packed on the device -> all_to_all -> unpack.
-    Returns (#records moving on ALL ranks, #received here).
+    Returns (#records moving on ALL ranks, #received here).  ``resume``: the engine carries each particle's resumable state
+    (AdvectionRK45, AdvectionDiffusionM1 / EM): a second buffer of 24-byte records goes along, split like the records.
 
     NCCL: the count matrix and the records stay on the device (records never touch the host).  gloo (CPU tests / two
     ranks sharing one GPU): the same device-side pack/unpack kernels, records staged through the host."""
@@ -198,28 +211,34 @@ def _exchange(eng, counts, dist, device):
         return 0, 0
     rc = m[:, rank]
     n_in = int(rc.sum())
+    sizes = (RECORD_BYTES, RESUME_BYTES) if resume else (RECORD_BYTES,)
+    sendbufs = [torch.empty(max(n_out, 1) * b, dtype=torch.uint8, device=device) for b in sizes]
+    if resume:
+        eng.migrate_pack_resume(sendbufs[0].data_ptr(), sendbufs[1].data_ptr(), n_out)
+    else:
+        eng.migrate_pack(sendbufs[0].data_ptr(), n_out)  # synchronises the engine stream before NCCL touches the buffer
     if nccl:
-        sendbuf = torch.empty(max(n_out, 1) * RECORD_BYTES, dtype=torch.uint8, device=device)
-        recvbuf = torch.empty(max(n_in, 1) * RECORD_BYTES, dtype=torch.uint8, device=device)
-        eng.migrate_pack(sendbuf.data_ptr(), n_out)  # synchronises the engine stream before NCCL touches the buffer
-        dist.all_to_all_single(recvbuf[: n_in * RECORD_BYTES], sendbuf[: n_out * RECORD_BYTES],
-                               output_split_sizes=[int(c) * RECORD_BYTES for c in rc],
-                               input_split_sizes=[int(c) * RECORD_BYTES for c in counts])  # fmt: skip
+        recvbufs = [torch.empty(max(n_in, 1) * b, dtype=torch.uint8, device=device) for b in sizes]
+        for sendbuf, recvbuf, b in zip(sendbufs, recvbufs, sizes, strict=True):
+            dist.all_to_all_single(recvbuf[: n_in * b], sendbuf[: n_out * b], output_split_sizes=[int(c) * b for c in rc],
+                                   input_split_sizes=[int(c) * b for c in counts])  # fmt: skip
         _sync(device)
-        eng.migrate_unpack(recvbuf.data_ptr(), n_in)
-        return total, n_in
-    sendbuf = torch.empty(max(n_out, 1) * RECORD_BYTES, dtype=torch.uint8, device=device)
-    eng.migrate_pack(sendbuf.data_ptr(), n_out)
-    host = sendbuf[: n_out * RECORD_BYTES].cpu().numpy()
-    offs = np.concatenate(([0], np.cumsum(counts))) * RECORD_BYTES
-    chunks = [host[offs[r] : offs[r + 1]].tobytes() for r in range(world)]
-    everyone = [None] * world
-    dist.all_gather_object(everyone, chunks)
-    got = b"".join(everyone[src][rank] for src in range(world))
-    assert len(got) == n_in * RECORD_BYTES
-    recvbuf = torch.frombuffer(bytearray(got) if got else bytearray(RECORD_BYTES), dtype=torch.uint8).to(device)
-    _sync(device)
-    eng.migrate_unpack(recvbuf.data_ptr(), n_in)
+    else:
+        recvbufs = []
+        for sendbuf, b in zip(sendbufs, sizes, strict=True):
+            host = sendbuf[: n_out * b].cpu().numpy()
+            offs = np.concatenate(([0], np.cumsum(counts))) * b
+            chunks = [host[offs[r] : offs[r + 1]].tobytes() for r in range(world)]
+            everyone = [None] * world
+            dist.all_gather_object(everyone, chunks)
+            got = b"".join(everyone[src][rank] for src in range(world))
+            assert len(got) == n_in * b
+            recvbufs.append(torch.frombuffer(bytearray(got) if got else bytearray(b), dtype=torch.uint8).to(device))
+        _sync(device)
+    if resume:
+        eng.migrate_unpack_resume(recvbufs[0].data_ptr(), recvbufs[1].data_ptr(), n_in)
+    else:
+        eng.migrate_unpack(recvbufs[0].data_ptr(), n_in)
     return total, n_in
 
 
@@ -254,7 +273,21 @@ def connect_p2p(dfs: DecomposedFieldSet, dist, capacity_records: int) -> bool:
     return dfs.p2p
 
 
+def _carries_resume(plan) -> bool:
+    """AdvectionRK45 and AdvectionDiffusionM1 / EM: a lane stopped mid-call continues on its new owner with its dt, next_dt and
+    iteration count, which travel with the particle."""
+    return plan.rk45 is not None or plan.advdiff is not None
+
+
 def _advect_args(eng, plan, dt, endtime, first, seed, rng_call, rounds):
+    if plan.rk45 is not None:
+        return eng.make_rk45_args(dt, endtime, *plan.rk45, next_dt_is_f32=plan.next_dt_dtype == np.float32, delete_on_error=True,
+                                  resume=not first, batch_levels=plan.batch_levels)  # fmt: skip
+    if plan.advdiff is not None:
+        # the iteration count travels with the particle and keys its Wiener increments: the single-GPU run's stream, unchanged by
+        # where the rounds cut the call (no round number in the call index)
+        return eng.make_advdiff_args(dt=dt, endtime=endtime, delete_on_error=True, seed=seed, rng_call=rng_call, resume=not first,
+                                     batch_levels=plan.batch_levels, **plan.advdiff)  # fmt: skip
     # fused DiffusionUniformKh: the Wiener increments are keyed by (seed; particle id, iteration of the launch, call index).  Every
     # migration round is a new launch on every rank (the round count is global), so the round number joins the call index and no
     # particle ever draws the same increment twice, wherever it migrates.  (The stream differs from a single-GPU run's, whose
@@ -309,6 +342,7 @@ def run_decomposed_p2p(dfs: DecomposedFieldSet, plan, dt: float, endtime: float,
     stats = dict(rounds=0, migrated=0, particle_steps=0, kernel_ms=0.0, exchange_ms=0.0, transport="peer memory (in-kernel)")
     for _ in range(max_rounds):
         rep = _advect_round(dfs, _advect_args(eng, plan, dt, endtime, stats["rounds"] == 0, seed, rng_call, stats["rounds"]), sign)
+        stats["max_iters_done"] = max(stats.get("max_iters_done", 0), rep["max_iters_done"])
         t0 = time.perf_counter()
         flags = torch.tensor([float(rep["n_migrate"]), float(rep["max_state"] == 99)], dtype=torch.float64,
                              device=device if dist.get_backend() == "nccl" else "cpu")
@@ -325,7 +359,19 @@ def run_decomposed_p2p(dfs: DecomposedFieldSet, plan, dt: float, endtime: float,
             raise RuntimeError("halo violation: a stage position left the owned+halo columns; increase halo_cells or reduce dt")
         if moved == 0 and not (dfs.fs.time_window is not None and _slide_in_lockstep(dfs, rep, sign, dist, device)):
             break
+    _finish_call(dfs, plan, dt, endtime, dist, device, stats)
     return stats
+
+
+def _finish_call(dfs, plan, dt, endtime, dist, device, stats):
+    """AdvectionRK45: the batch-level dt clamp of the particles that left the loop early needs the call's iteration count over
+    every rank and round -- once, on every rank, after the last round."""
+    if plan.rk45 is not None:
+        dfs.engine.rk45_finalize(dt, endtime, int(allreduce_max(stats.get("max_iters_done", 0), dist, _collective_device(dist, device))))
+
+
+def _collective_device(dist, device):
+    return device if dist.get_backend() == "nccl" else "cpu"
 
 
 def run_decomposed_resident(dfs: DecomposedFieldSet, plan, dt: float, endtime: float, dist, max_rounds=100000, seed=0, rng_call=1):
@@ -345,7 +391,7 @@ def run_decomposed_resident(dfs: DecomposedFieldSet, plan, dt: float, endtime: f
     for _ in range(max_rounds):
         t0 = time.perf_counter()
         counts = eng.migrate_count()
-        total, _ = _exchange(eng, counts, dist, device)
+        total, _ = _exchange(eng, counts, dist, device, resume=_carries_resume(plan))
         stats["exchange_ms"] += 1e3 * (time.perf_counter() - t0)
         stats["migrated"] += int(counts.sum())
         if total == 0 and not first and not (dfs.fs.time_window is not None and _slide_in_lockstep(dfs, rep, sign, dist, device)):
@@ -355,46 +401,87 @@ def run_decomposed_resident(dfs: DecomposedFieldSet, plan, dt: float, endtime: f
         stats["rounds"] += 1
         stats["particle_steps"] += rep["particle_steps"]
         stats["kernel_ms"] += rep["kernel_ms"]
+        stats["max_iters_done"] = max(stats.get("max_iters_done", 0), rep["max_iters_done"])
         if rep["max_state"] == 99:  # every rank raises in the same round or the next count exchange would hang: agree first
             stats["halo_violation"] = True
         if allreduce_max(float(rep["max_state"] == 99), dist, device) > 0:
             raise RuntimeError("halo violation: a stage position left the owned+halo columns; increase halo_cells or reduce dt")
+    _finish_call(dfs, plan, dt, endtime, dist, device, stats)
     return stats
 
 
-def decomposed_plan(dfs: DecomposedFieldSet, kernels):
+def decomposed_plan(dfs: DecomposedFieldSet, kernels, pdata: dict | None = None):
+    """The kernel list lowered for mode D: one of the fused fixed-step schemes (optionally with DiffusionUniformKh),
+    ``[AdvectionRK45, DeleteParticle]`` (``pdata`` must then hold ``next_dt``) or ``[AdvectionDiffusionM1 | EM, DeleteParticle]``."""
+    from types import SimpleNamespace
+
     from .particleset import KernelPlan
 
-    plan = KernelPlan(kernels, dfs.fs)
+    # (the particle variables stand in for the ParticleClass: RK45 needs next_dt)
+    pclass = SimpleNamespace(variables=[SimpleNamespace(name=k) for k in (pdata or {})])
+    plan = KernelPlan(kernels, dfs.fs, pclass)
+    if plan.stepwise:
+        raise NotImplementedError("domain-decomposed execution runs one built-in kernel -- a fixed-step advection scheme (optionally "
+                                  "with DiffusionUniformKh), AdvectionRK45 or AdvectionDiffusionM1 / EM -- followed by DeleteParticle; "
+                                  "user kernels and other mixes run on one GPU")  # fmt: skip
     if not plan.delete_on_error:
         raise NotImplementedError("domain-decomposed execution needs the DeleteParticle handler (errors cannot be replayed "
                                   "step-exactly across ranks)")  # fmt: skip
+    plan.batch_levels = 0  # the call's batch-level bits (execute_decomposed sets them for the kernels that carry their iterations)
+    plan.next_dt_dtype = np.dtype(pdata["next_dt"].dtype) if plan.rk45 is not None else None
     return plan
 
 
-def upload_decomposed(dfs: DecomposedFieldSet, pdata: dict, dt: float):
+def upload_decomposed(dfs: DecomposedFieldSet, pdata: dict, dt: float, plan=None):
+    """Make ``pdata`` this rank's resident set.  AdvectionRK45 keeps every particle's dt and next_dt (the reference never resets dt
+    in RK45 mode); the kernels that continue a lane on another rank get their resumable-state columns."""
     from .statuscodes import StatusCode
 
     pdata["state"][:] = StatusCode.Evaluate
-    pdata["dt"][:] = dt
+    rk45 = plan is not None and plan.rk45 is not None
+    if not rk45:
+        pdata["dt"][:] = dt
     dfs.engine.upload_particles(pdata, np.ascontiguousarray(pdata["ei"][:, -1]))
+    if plan is not None and _carries_resume(plan):
+        dfs.engine.upload_resume(len(pdata["x"]), dt=pdata["dt"] if rk45 else None, next_dt=pdata["next_dt"] if rk45 else None)
 
 
-def download_decomposed(dfs: DecomposedFieldSet, dt: float, ngrids=1) -> dict:
+def download_decomposed(dfs: DecomposedFieldSet, dt: float, ngrids=1, plan=None) -> dict:
+    """This rank's resident set (deleted particles dropped); with AdvectionRK45 each particle's own dt and next_dt."""
     from .statuscodes import StatusCode
 
     out = dfs.engine.download_all(ngrids=ngrids)
-    out["dt"][:] = dt
+    if plan is not None and plan.rk45 is not None:
+        out["dt"][:], ndt, _ = dfs.engine.download_resume(len(out["x"]))
+        out["next_dt"] = ndt.astype(plan.next_dt_dtype)
+    else:
+        out["dt"][:] = dt
     keep = out["state"] != StatusCode.Delete
     return {k: v[keep] for k, v in out.items()}
+
+
+def _global_batch_levels(dfs, pdata, dt, endtime, dist, device) -> int:
+    """The reference's batch-level bits of the call's first evaluation (particleset._batch_levels) over the WHOLE set -- every rank's
+    shard -- so that the first-iteration rule of the kernels that count their iterations across ranks is the single-GPU one."""
+    import torch
+
+    from .particleset import _batch_levels
+
+    sign = 1 if dt > 0 else -1
+    bits = _batch_levels(dfs.fs, pdata, sign * (endtime - pdata["t"]) >= 0) if len(pdata["t"]) else 0
+    v = torch.tensor([float(bits & 1), float(bits & 2)], dtype=torch.float64, device=_collective_device(dist, device))
+    dist.all_reduce(v, op=dist.ReduceOp.MAX)
+    return int(v[0].item() > 0) | (2 if v[1].item() > 0 else 0)
 
 
 def execute_decomposed(dfs: DecomposedFieldSet, pdata: dict, kernels, dt: float, endtime: float, dist, max_rounds=100000, seed=0,
                        rng_call=1):
     """``Kernel.execute`` over a domain-decomposed field: ``pdata`` is ANY shard of the particle set (it is
     routed to the owners first).  Returns (local particle dict after the call, stats)."""
-    plan = decomposed_plan(dfs, kernels)
-    upload_decomposed(dfs, pdata, dt)
+    plan = decomposed_plan(dfs, kernels, pdata)
+    upload_decomposed(dfs, pdata, dt, plan)
+    if _carries_resume(plan):
+        plan.batch_levels = _global_batch_levels(dfs, pdata, dt, endtime, dist, _engine_memory_device(dfs.device))
     if dfs.fs.time_window is not None:
         # first window: where the earliest (latest, backward in time) particle of ANY rank starts -- the same on every rank
         import torch
@@ -408,4 +495,4 @@ def execute_decomposed(dfs: DecomposedFieldSet, pdata: dict, kernels, dt: float,
         if np.isfinite(float(v.item())):
             dfs.fs.slide_window(dfs.device, sign * float(v.item()), sign)
     stats = run_decomposed_resident(dfs, plan, dt, endtime, dist, max_rounds=max_rounds, seed=seed, rng_call=rng_call)
-    return download_decomposed(dfs, dt, ngrids=pdata["ei"].shape[1]), stats
+    return download_decomposed(dfs, dt, ngrids=pdata["ei"].shape[1], plan=plan), stats

@@ -224,16 +224,43 @@ class Engine:
                           int(bool(hint_all_zero)), int(bool(resume)), int(bool(kernels_only)), int(batch_levels))  # fmt: skip
 
     def advect(self, args) -> dict:
-        """``Kernel.execute`` on the device: ``args`` from :meth:`make_args` (pb_advect) or :meth:`make_advdiff_args`
-        (pb_advect_diffusion: AdvectionDiffusionM1 / EM)."""
-        from ._lib import AdvDiffArgs
+        """``Kernel.execute`` on the device: ``args`` from :meth:`make_args` (pb_advect), :meth:`make_advdiff_args`
+        (pb_advect_diffusion: AdvectionDiffusionM1 / EM) or :meth:`make_rk45_args` (pb_advect_rk45_resident_async: AdvectionRK45 on
+        the resident dt / next_dt / iteration columns)."""
+        from ._lib import AdvDiffArgs, Rk45Args
 
         rep = Report()
         if isinstance(args, AdvDiffArgs):
             check(self._lib.pb_advect_diffusion(self._h, C.byref(args), C.byref(rep)))
+        elif isinstance(args, Rk45Args):
+            check(self._lib.pb_advect_rk45_resident_async(self._h, C.byref(args)))
+            check(self._lib.pb_last_report(self._h, C.byref(rep)))
         else:
             check(self._lib.pb_advect(self._h, C.byref(args), C.byref(rep)))
         return _report_dict(rep)
+
+    @staticmethod
+    def make_rk45_args(dt, endtime, tol, min_dt, max_dt, *, next_dt_is_f32=True, delete_on_error=False, resume=False, batch_levels=0):
+        from ._lib import Rk45Args
+
+        return Rk45Args(float(dt), float(endtime), float(tol), float(min_dt), float(max_dt), -1, int(next_dt_is_f32),
+                        int(delete_on_error), 0, int(bool(resume)), 0, int(batch_levels))  # fmt: skip
+
+    def rk45_finalize(self, dt, endtime, total_iters):
+        """The batch-level dt clamp of the particles that left the RK45 loop before the call's ``total_iters`` iterations
+        (pb_rk45_finalize_resident), once after the last launch of a call on the resident columns."""
+        check(self._lib.pb_rk45_finalize_resident(self._h, float(dt), float(endtime), int(total_iters)))
+
+    def upload_resume(self, n, dt=None, next_dt=None, iters=None):
+        """Make each particle's resumable state -- dt, next_dt (float64), iteration count (int32) -- resident columns (None: zeros)."""
+        arrs = [None if a is None else np.ascontiguousarray(a, dtype=dt_) for a, dt_ in ((dt, np.float64), (next_dt, np.float64),
+                                                                                        (iters, np.int32))]  # fmt: skip
+        check(self._lib.pb_particles_upload_resume(self._h, int(n), *(ptr(a) for a in arrs)))
+
+    def download_resume(self, n) -> tuple:
+        dt, ndt, it = np.empty(n, dtype=np.float64), np.empty(n, dtype=np.float64), np.empty(n, dtype=np.int32)
+        check(self._lib.pb_particles_download_resume(self._h, int(n), ptr(dt), ptr(ndt), ptr(it)))
+        return dt, ndt, it
 
     @staticmethod
     def make_advdiff_args(scheme, dt, endtime, *, kh_slots, dres, deg2m_sq, delete_on_error=False, seed=0, rng_call=0, max_iters=-1,
@@ -271,10 +298,12 @@ class Engine:
 
     def advect_async(self, args):
         """:meth:`advect` without waiting for the kernel; :meth:`last_report` waits and returns the report."""
-        from ._lib import AdvDiffArgs
+        from ._lib import AdvDiffArgs, Rk45Args
 
         if isinstance(args, AdvDiffArgs):
             check(self._lib.pb_advect_diffusion_async(self._h, C.byref(args)))
+        elif isinstance(args, Rk45Args):
+            check(self._lib.pb_advect_rk45_resident_async(self._h, C.byref(args)))
         else:
             check(self._lib.pb_advect_async(self._h, C.byref(args)))
 
@@ -330,6 +359,13 @@ class Engine:
 
     def migrate_unpack(self, recvbuf_ptr: int, n_in: int):
         check(self._lib.pb_migrate_unpack(self._h, C.c_void_p(recvbuf_ptr), int(n_in)))
+
+    # the same with the resumable state resident: a second buffer of 24-byte records at the same indices
+    def migrate_pack_resume(self, sendbuf_ptr: int, resume_ptr: int, capacity_records: int):
+        check(self._lib.pb_migrate_pack_resume(self._h, C.c_void_p(sendbuf_ptr), C.c_void_p(resume_ptr), int(capacity_records)))
+
+    def migrate_unpack_resume(self, recvbuf_ptr: int, resume_ptr: int, n_in: int):
+        check(self._lib.pb_migrate_unpack_resume(self._h, C.c_void_p(recvbuf_ptr), C.c_void_p(resume_ptr), int(n_in)))
 
     # in-kernel migration over peer memory (pb_migrate_p2p_*, include/parcels_b200.h)
     def migrate_p2p_init(self, capacity_records: int):

@@ -30,6 +30,14 @@ ap.add_argument("--time-window", type=int, default=0, help="time-slab streaming 
 ap.add_argument("--nt", type=int, default=3, help="time levels of the synthetic field (one day apart)")
 ap.add_argument("--runtime", type=float, default=86400.0)
 ap.add_argument("--diffusion", action="store_true", help="fused DiffusionUniformKh on a field at rest: statistical check (Var = 2 K t)")
+ap.add_argument("--kernel", default="rk4_3d", choices=["rk4_3d", "rk45", "m1", "em"],
+                help="rk45 / m1 / em: [AdvectionRK45 | AdvectionDiffusionM1 | EM, DeleteParticle] (scripts/decomposed_kernels.py)")
+ap.add_argument("--mesh", default="spherical", choices=["spherical", "flat"])
+ap.add_argument("--backward", action="store_true")
+ap.add_argument("--delayed", action="store_true", help="releases at three different times")
+ap.add_argument("--max-dt", type=float, default=3600.0, help="RK45_max_dt")
+ap.add_argument("--dres", type=float, default=0.05, help="fieldset.dres of M1 / EM (degrees or mesh units)")
+ap.add_argument("--rk45-tol", type=float, default=100.0, help="RK45_tol in metres")
 a = ap.parse_args()
 rank, world = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])
 dev = 0 if a.same_gpu else int(os.environ.get("LOCAL_RANK", rank))
@@ -70,6 +78,35 @@ if a.diffusion:
               and abs(float(np.mean(merged["x"]))) < 5 * sigma / np.sqrt(n) and tot > n / 4)  # fmt: skip
         print(f"decomposed diffusion ({world} ranks): {len(merged['x'])} particles, {int(tot)} migrations, rounds={stats['rounds']}, "
               f"std x {sx:.4f} y {sy:.4f} expected {sigma:.4f} -> {'PASS statistics' if ok else 'FAIL'}")
+    dist.barrier()
+    dist.destroy_process_group()
+    sys.exit(0 if ok else 1)
+if a.kernel != "rk4_3d":
+    sys.path.insert(0, os.path.join(ROOT, "scripts"))
+    import decomposed_kernels
+
+    case = decomposed_kernels.make_case(a.kernel, mesh=a.mesh, n=n, nt=a.nt, runtime=a.runtime, backward=a.backward,
+                                        delayed=a.delayed or bool(a.time_window), max_dt=a.max_dt, dres=a.dres, tol=a.rk45_tol)  # fmt: skip
+    dfs = decomposed_kernels.decomposed_fieldset(case, rank, world, halo=a.halo, time_window=a.time_window or None, device=dev)
+    if p2p:
+        D.connect_p2p(dfs, dist, a.inbox or n)
+    try:
+        out, stats = D.execute_decomposed(dfs, D.shard_particles(case["full"], rank, world), case["kernels"], case["dt"],
+                                          case["endtime"], dist, seed=case["seed"])  # fmt: skip
+    except RuntimeError as e:  # (every rank raises a halo violation in the same round)
+        print(f"rank {rank}: RuntimeError: {e}")
+        dist.destroy_process_group()
+        sys.exit(3)
+    tot = D.allreduce_sum(stats["migrated"], dist, device="cpu" if a.same_gpu else f"cuda:{dev}")
+    merged = D.gather_particles(out, dist, dst=0)
+    ok = True
+    if rank == 0:
+        ref = decomposed_kernels.reference(case, device=dev)
+        ok, msgs = decomposed_kernels.compare(merged, ref, a.kernel)
+        print("\n".join(msgs))
+        print(f"decomposed {a.kernel} ({world} ranks, backend={dist.get_backend()}, {a.mesh}{', backward' if a.backward else ''}): "
+              f"{len(ref['x'])} of {n} left, {int(tot)} migrations, rounds={stats['rounds']}, transport={stats['transport']}"
+              + (f", time window {a.time_window} of {a.nt} levels" if a.time_window else "") + f" -> {'PASS bit-exact' if ok else 'FAIL'}")  # fmt: skip
     dist.barrier()
     dist.destroy_process_group()
     sys.exit(0 if ok else 1)

@@ -15,6 +15,7 @@ sys.path[:0] = [ROOT, os.path.join(ROOT, "tests"), os.path.join(ROOT, "scripts")
 import numpy as np
 
 import bench
+import decomposed_kernels
 import parcels_b200 as pb
 import thread_ranks
 from parcels_b200 import distributed as D
@@ -30,8 +31,16 @@ def main():
     ap.add_argument("--nt", type=int, default=3)
     ap.add_argument("--runtime", type=float, default=86400.0)
     ap.add_argument("--backward", action="store_true")
+    ap.add_argument("--kernel", default="rk4_3d", choices=["rk4_3d", *decomposed_kernels.KERNELS],
+                    help="rk45 / m1 / em: [AdvectionRK45 | AdvectionDiffusionM1 | EM, DeleteParticle] (scripts/decomposed_kernels.py)")
+    ap.add_argument("--mesh", default="spherical", choices=["spherical", "flat"])
+    ap.add_argument("--delayed", action="store_true", help="releases at three different times")
+    ap.add_argument("--halo", type=int, default=3)
+    ap.add_argument("--max-dt", type=float, default=3600.0, help="RK45_max_dt")
     a = ap.parse_args()
     world, n = a.world, a.particles
+    if a.kernel != "rk4_3d":
+        return kernel_case(a)
     f = bench.c2_field(nx=120, ny=60, nz=12, nt=a.nt)
     f["U"] *= np.float32(40.0)
     f["V"] *= np.float32(40.0)
@@ -72,6 +81,31 @@ def main():
     print(f"decomposed({world} thread ranks): {len(ref['x'])} survivors, {migrated} migrations, rounds={stats[0]['rounds']}, "
           f"transport={stats[0]['transport']}" + (f", time window {a.time_window} of {a.nt} levels" if a.time_window else "")
           + f" -> {'PASS bit-exact' if ok else 'FAIL'}")  # fmt: skip
+    return 0 if ok else 1
+
+
+def kernel_case(a):
+    case = decomposed_kernels.make_case(a.kernel, mesh=a.mesh, n=a.particles, nt=a.nt, runtime=a.runtime, backward=a.backward,
+                                        delayed=a.delayed or bool(a.time_window), max_dt=a.max_dt)  # fmt: skip
+    world, n = a.world, a.particles
+    slabs = [decomposed_kernels.decomposed_fieldset(case, r, world, halo=a.halo, time_window=a.time_window or None) for r in range(world)]
+    bases = [s.engine.migrate_p2p_init(a.inbox or n)[1] for s in slabs]
+    for s in slabs:
+        s.engine.migrate_p2p_connect(local_bases=bases)
+        s.p2p = True
+    thread_ranks.serialise_engine_calls()
+    full = case["full"]
+    res = thread_ranks.run_ranks(world, lambda r, dist: D.execute_decomposed(slabs[r], D.shard_particles(full, r, world), case["kernels"],
+                                                                             case["dt"], case["endtime"], dist, seed=case["seed"]))  # fmt: skip
+    outs, stats = [o for o, _ in res], [s for _, s in res]
+    merged = {k: np.concatenate([o[k] for o in outs], axis=0) for k in outs[0]}
+    ref = decomposed_kernels.reference(case)
+    ok, msgs = decomposed_kernels.compare(merged, ref, a.kernel)
+    print("\n".join(msgs))
+    migrated = sum(s["migrated"] for s in stats)
+    print(f"decomposed {a.kernel} ({world} thread ranks, {a.mesh}{', backward' if a.backward else ''}): {len(ref['x'])} of {n} left, "
+          f"{migrated} migrations, rounds={stats[0]['rounds']}, transport={stats[0]['transport']}"
+          + (f", time window {a.time_window} of {a.nt} levels" if a.time_window else "") + f" -> {'PASS bit-exact' if ok else 'FAIL'}")  # fmt: skip
     return 0 if ok else 1
 
 
