@@ -463,6 +463,16 @@ int32_t pb_debug_math(pb_engine* e, int32_t op, int64_t n, const double* a, cons
 /* The device cell table of axis `axis` (0 lon, 1 lat, 2 depth, 3 time) of a float64 rectilinear grid: `cells` records of 4 doubles
  * {lo, hi, 1 / (hi - lo), 0} into `out`; `cells` must be the axis' node count - 1.  PB_ERR_INVALID when there is no such table. */
 int32_t pb_debug_axis_cells(pb_engine* e, int32_t axis, int64_t cells, double* out);
+/* Threads per block the particle kernels of a family are launched with (as the library was built): the lane / warp / block a
+ * particle runs in is its storage position's, i.e. position % block and position / block.  PB_ERR_INVALID for an unknown family. */
+enum pb_launch_family {
+    PB_BLOCK_AGRID_FAST = 0, /* the specialised RK4 kernel (afast.cu) */
+    PB_BLOCK_AGRID = 1,      /* the generic A-grid kernels (agrid.cu) */
+    PB_BLOCK_CGRID = 2,      /* rectilinear and curvilinear C-grids (cgrid.cu) */
+    PB_BLOCK_CURV_AGRID = 3, /* XLinear_Velocity on curvilinear grids (curva.cu) */
+    PB_BLOCK_SAMPLE_FLAGS = 4 /* the batch-level lenT / lenZ pre-pass of pb_sample_velocity / pb_sample_scalar */
+};
+int32_t pb_debug_launch_block(int32_t family);
 
 /* ---- host-side passes of Kernel.execute / ParticleSet.execute over the particle columns, multi-threaded ----------------
  * The reference makes a few whole-column passes per call on the host: `pset._data["dt"][:] = dt` (_core/particleset.py:405,

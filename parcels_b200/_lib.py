@@ -169,6 +169,7 @@ SYMBOLS = {
     "pb_debug_normals": (C.c_int32, [_P, C.c_uint64, C.c_uint64, C.c_int64, C.c_int64, _P, _P]),
     "pb_debug_math": (C.c_int32, [_P, C.c_int32, C.c_int64, _P, _P, _P]),
     "pb_debug_axis_cells": (C.c_int32, [_P, C.c_int32, C.c_int64, _P]),
+    "pb_debug_launch_block": (C.c_int32, [C.c_int32]),
     "pb_host_fill_f64": (C.c_int32, [_P, C.c_int64, C.c_double]),
     "pb_host_fill_i32": (C.c_int32, [_P, C.c_int64, C.c_int32]),
     "pb_host_min_max_f64": (C.c_int32, [_P, C.c_int64, _P, _P, _P]),

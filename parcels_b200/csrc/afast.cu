@@ -585,6 +585,8 @@ static cudaError_t launch_fast1(const AdvectParams& p, int sched, cudaStream_t s
     return sched == 2 ? launch_fast2<NC, HZ, 2, false>(p, s) : launch_fast2<NC, HZ, 1, false>(p, s);
 }
 
+int afast_launch_block() { return PB_FAST_BLOCK; }
+
 cudaError_t launch_agrid_fast(const AdvectParams& p, int nc, int sched, cudaStream_t s) {
     const bool hz = p.g.nz >= 2;
     if (nc == 3) return launch_fast1<3, true>(p, sched, s);

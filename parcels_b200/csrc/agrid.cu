@@ -1,6 +1,8 @@
 // agrid.cu -- launchers of the XLinear_Velocity A-grid kernels (the headline hot path); device code in agrid.cuh
 #include "agrid.cuh"
 
+int agrid_launch_block() { return PB_BLOCK; }
+
 template <class A, class D, bool HT, int NC>
 static cudaError_t launch1(const AdvectParams& p, cudaStream_t s) {
     const int block = PB_BLOCK;

@@ -23,9 +23,12 @@ cudaError_t launch_sample_scalar_curv(const SampleParams& p, int mode, bool coor
     return data_f64 ? scalar_curv_ad<float, double>(p, mode, has_time, s) : scalar_curv_ad<float, float>(p, mode, has_time, s);
 }
 
+static constexpr int ADVECT_BLOCK = 128;
+int cgrid_launch_block() { return ADVECT_BLOCK; }
+
 template <class Policy>
 static cudaError_t launch_policy(const AdvectParams& p, cudaStream_t s) {
-    const int block = 128;
+    const int block = ADVECT_BLOCK;
     const long long grid = (p.P.n + block - 1) / block;
     // (advection-only launches carry neither the Philox / Box-Muller code nor its registers in the time loop)
     if (Policy::RUNTIME_DTYPE && !p.diffusion) advect_kernel<Policy, false><<<(unsigned)grid, block, 0, s>>>(p);

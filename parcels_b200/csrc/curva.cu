@@ -3,9 +3,12 @@
 // (interpolators/_xinterpolators.py:112-190).  Its own translation unit: the C-grid kernels of cgrid.cu stay the measured builds.
 #include "cgrid.cuh"
 
+static constexpr int ADVECT_BLOCK = 128;
+int curva_launch_block() { return ADVECT_BLOCK; }
+
 template <class Policy>
 static cudaError_t launch_policy(const AdvectParams& p, cudaStream_t s) {
-    const int block = 128;
+    const int block = ADVECT_BLOCK;
     advect_kernel<Policy><<<(unsigned)((p.P.n + block - 1) / block), block, 0, s>>>(p);
     return cudaGetLastError();
 }

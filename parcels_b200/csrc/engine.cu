@@ -1011,11 +1011,12 @@ static int32_t check_fields(pb_engine* e, int nc) {
 }
 
 // pre-pass of a sampling call: the reference's batch-level lenT / lenZ into the device word `flags` (see sample_flags_kernel)
+static constexpr int SAMPLE_FLAGS_BLOCK = 256;
 static int32_t launch_sample_flags(pb_engine* e, SampleParams& sp, bool has_time, int* flags) {
     CK(cudaMemsetAsync(flags, 0, sizeof(int), e->stream));
-    const unsigned grid = (unsigned)((sp.n + 255) / 256);
-    if (e->coord_f64) sample_flags_kernel<double><<<grid, 256, 0, e->stream>>>(sp, has_time ? 1 : 0, flags);
-    else sample_flags_kernel<float><<<grid, 256, 0, e->stream>>>(sp, has_time ? 1 : 0, flags);
+    const unsigned grid = (unsigned)((sp.n + SAMPLE_FLAGS_BLOCK - 1) / SAMPLE_FLAGS_BLOCK);
+    if (e->coord_f64) sample_flags_kernel<double><<<grid, SAMPLE_FLAGS_BLOCK, 0, e->stream>>>(sp, has_time ? 1 : 0, flags);
+    else sample_flags_kernel<float><<<grid, SAMPLE_FLAGS_BLOCK, 0, e->stream>>>(sp, has_time ? 1 : 0, flags);
     CK(cudaGetLastError());
     sp.batch_flags = flags;
     return PB_OK;
@@ -1584,6 +1585,17 @@ int32_t pb_debug_math(pb_engine* e, int32_t op, int64_t n, const double* a, cons
     cudaFree(d_b);
     cudaFree(d_out);
     return PB_OK;
+}
+
+int32_t pb_debug_launch_block(int32_t family) {
+    switch (family) {
+        case PB_BLOCK_AGRID_FAST: return afast_launch_block();
+        case PB_BLOCK_AGRID: return agrid_launch_block();
+        case PB_BLOCK_CGRID: return cgrid_launch_block();
+        case PB_BLOCK_CURV_AGRID: return curva_launch_block();
+        case PB_BLOCK_SAMPLE_FLAGS: return SAMPLE_FLAGS_BLOCK;
+        default: return fail(PB_ERR_INVALID, "unknown kernel family %d", family);
+    }
 }
 
 

@@ -451,3 +451,12 @@ class Engine:
         out = np.empty((nodes - 1, 4), dtype=np.float64)
         check(self._lib.pb_debug_axis_cells(self._h, self.AXES[axis], nodes - 1, ptr(out)))
         return out
+
+    LAUNCH_FAMILIES = {"agrid_fast": 0, "agrid": 1, "cgrid": 2, "curv_agrid": 3, "sample_flags": 4}  # enum pb_launch_family
+
+    def debug_launch_block(self, family):
+        """Threads per block of the particle kernels of `family` (see pb_debug_launch_block)."""
+        block = self._lib.pb_debug_launch_block(self.LAUNCH_FAMILIES[family])
+        if block <= 0:
+            check(block)
+        return block

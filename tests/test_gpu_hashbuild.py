@@ -47,3 +47,23 @@ def test_host_table_route_gives_identical_trajectories():
     ps.execute([pb.AdvectionRK4, pb.DeleteParticle], dt=c["dt"], **c["segments"][0])
     for k in ("particle_id", "state", "t", "ei", "x", "y"):
         np.testing.assert_array_equal(ps._data[k], ps_dev._data[k], err_msg=k)
+
+
+def test_device_table_equals_host_table_at_tens_of_millions_of_entries():
+    """The device build's cub scan and radix sort at a size no other case reaches: a 3000 x 4000-node spherical mesh (about
+    1.2e7 faces, 2.7e7 table entries, well above ORCA025's 1.27e7).  Under the host simulation a 300 x 400 mesh (logic only)."""
+    import os
+
+    import parcels_b200 as pb
+
+    ny, nx = (300, 400) if os.environ.get("PB_HOSTSIM_TEST") == "1" else (3000, 4000)
+    lon, lat = cases.curv_mesh(ny, nx, True, np.dtype("f8"))
+    U = np.zeros((1, 1, ny, nx), dtype=np.float32)
+    fs = pb.FieldSet.from_arrays(lon=lon, lat=lat, U=U, V=U, mesh="spherical", interp_method="cgrid_velocity")
+    dev = fs.engine(0).hash_table()
+    host = build_spatial_hash(lon, lat, True, table=True)
+    if ny == 3000:
+        assert host["n_entries"] > 2.5e7
+    assert len(dev["faces"]) == host["n_entries"]
+    for k in ("keys", "starts", "counts", "faces"):
+        np.testing.assert_array_equal(dev[k], host[k], err_msg=k)
