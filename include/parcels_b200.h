@@ -454,10 +454,14 @@ int32_t pb_debug_normals(pb_engine* e, uint64_t seed, uint64_t rng_call, int64_t
  *   PB_MATH_DIV_BY_CACHED         div_by_cached(a[i], b[i], r), r  (common.cuh; r = 1.0 / b[i] computed on the device)
  *   PB_MATH_DIV_BY_CACHED_GUARDED div_by_cached_guarded(a[i], b[i], r), r
  *   PB_MATH_BOX_MULLER_F32        zx, zy of box_muller_f32((uint32_t)a[i], (uint32_t)b[i])  (the two Philox words)
- * b may be NULL for the first three. */
+ *   PB_MATH_COSF                  cosf_ool((float)a[i]), 0         (cgrid.cuh: CUDA's float32 cosf; the float32 result widened)
+ *   PB_MATH_SINF                  sinf_ool((float)a[i]), 0         (cgrid.cuh: CUDA's float32 sinf)
+ *   PB_MATH_COS                   cos_ool(a[i]), 0                 (cgrid.cuh: CUDA's float64 cos -- the per-cell table, sinx)
+ *   PB_MATH_SIN                   sin_ool(a[i]), 0                 (cgrid.cuh: CUDA's float64 sin)
+ * b may be NULL for every op but the three binary ones (DIV_BY_CACHED, DIV_BY_CACHED_GUARDED, BOX_MULLER_F32). */
 enum pb_math_op {
     PB_MATH_COS_NP = 0, PB_MATH_SIN_LAT = 1, PB_MATH_SINCOS_LON = 2, PB_MATH_DIV_BY_CACHED = 3, PB_MATH_DIV_BY_CACHED_GUARDED = 4,
-    PB_MATH_BOX_MULLER_F32 = 5
+    PB_MATH_BOX_MULLER_F32 = 5, PB_MATH_COSF = 6, PB_MATH_SINF = 7, PB_MATH_COS = 8, PB_MATH_SIN = 9
 };
 int32_t pb_debug_math(pb_engine* e, int32_t op, int64_t n, const double* a, const double* b, double* out);
 /* The device cell table of axis `axis` (0 lon, 1 lat, 2 depth, 3 time) of a float64 rectilinear grid: `cells` records of 4 doubles

@@ -11,6 +11,8 @@ from __future__ import annotations
 
 import numpy as np
 
+from . import trig
+
 GRID_SEARCH_ERROR = -3
 
 # ----------------------------------------------------------------------------------------------
@@ -45,8 +47,8 @@ def bilinear_inverse(px, py, xq, yq):
 
 def project_cell_and_query(clon, clat, x, y):
     """_core/index_search.py:180-239: corners and query on the cell's own tangent plane."""
-    cX, cY, cZ = latlon_rad_to_xyz(np.deg2rad(clat), np.deg2rad(clon))
-    qX, qY, qZ = latlon_rad_to_xyz(np.deg2rad(np.asarray(y, dtype=float)), np.deg2rad(np.asarray(x, dtype=float)))
+    cX, cY, cZ = trig.current().curv_corners(np.deg2rad(clat), np.deg2rad(clon))
+    qX, qY, qZ = trig.current().curv_query(np.deg2rad(np.asarray(y, dtype=float)), np.deg2rad(np.asarray(x, dtype=float)))
     ux = (cX[1] + cX[2]) - (cX[0] + cX[3])
     uy = (cY[1] + cY[2]) - (cY[0] + cY[3])
     uz = (cZ[1] + cZ[2]) - (cZ[0] + cZ[3])
@@ -204,7 +206,7 @@ class OHash:
     def query(self, y, x):  # :389-535
         y, x = np.asarray(y), np.asarray(x)
         if self.grid.spherical:
-            qx, qy, qz = latlon_rad_to_xyz(np.deg2rad(y), np.deg2rad(x))
+            qx, qy, qz = trig.current().hash_query(np.deg2rad(y), np.deg2rad(x))
         else:
             qx, qy, qz = x, y, np.zeros_like(x)
         codes = morton3(*quantize(qx, qy, qz, self.box, self.bitwidth)).ravel()
@@ -247,7 +249,8 @@ def get_hash(grid):
 
 def search_indices_curvilinear_2d(grid, y, x, yi=None, xi=None):
     """_core/index_search.py:242-295."""
-    if np.any(xi):
+    hinted = bool(np.any(xi))
+    if hinted:
         inside, coords = point_in_cell(grid, y, x, yi, xi)
         y_check, x_check = y[inside == 0], x[inside == 0]
         miss = np.where(inside == 0)[0]
@@ -262,6 +265,8 @@ def search_indices_curvilinear_2d(grid, y, x, yi=None, xi=None):
         coords[miss, :] = cq
         yi[miss] = yq
         xi[miss] = xq
+    if not hinted:
+        coords = trig.current().unhinted_coords(coords)
     return yi, coords[:, 1], xi, coords[:, 0]
 
 
@@ -277,7 +282,7 @@ def _edge_length(lat1, lat2, lon1, lon2, spherical, lat, deg2m):
     """_core/utils/interpolation.py:178-185 (``_geodetic_distance``)."""
     if spherical:
         rad = np.pi / 180.0
-        return np.sqrt(((lon2 - lon1) * deg2m * np.cos(rad * lat)) ** 2 + ((lat2 - lat1) * deg2m) ** 2)
+        return np.sqrt(((lon2 - lon1) * deg2m * trig.current().edge_length(rad * lat)) ** 2 + ((lat2 - lat1) * deg2m) ** 2)
     return np.sqrt((lon2 - lon1) ** 2 + (lat2 - lat1) ** 2)
 
 
@@ -285,10 +290,11 @@ def _jacobian(py, px, eta, xsi):
     """_core/utils/interpolation.py:188-198."""
     dphidxsi = np.column_stack([eta - 1, 1 - eta, eta, -eta])
     dphideta = np.column_stack([xsi - 1, -xsi, xsi, 1 - xsi])
-    dxdxsi = np.einsum("ij,ji->i", dphidxsi, px)
-    dxdeta = np.einsum("ij,ji->i", dphideta, px)
-    dydxsi = np.einsum("ij,ji->i", dphidxsi, py)
-    dydeta = np.einsum("ij,ji->i", dphideta, py)
+    rows = trig.current().einsum_rows
+    dxdxsi = rows(dphidxsi, px)
+    dxdeta = rows(dphideta, px)
+    dydxsi = rows(dphidxsi, py)
+    dydeta = rows(dphideta, py)
     return dxdxsi * dydeta - dxdeta * dydxsi
 
 
@@ -321,10 +327,11 @@ def cgrid_velocity(fs, pos, gp):
         px[1:] = np.where(px[1:] - px[0] > 180, px[1:] - 360, px[1:])
         px[1:] = np.where(-px[1:] + px[0] > 180, px[1:] + 360, px[1:])
     sph, d2m = grid.spherical, grid.deg2m
-    c1 = _edge_length(py[0], py[1], px[0], px[1], sph, np.einsum("ij,ji->i", _phi2d(0.0, xsi), py), d2m)
-    c2 = _edge_length(py[1], py[2], px[1], px[2], sph, np.einsum("ij,ji->i", _phi2d(eta, 1.0), py), d2m)
-    c3 = _edge_length(py[2], py[3], px[2], px[3], sph, np.einsum("ij,ji->i", _phi2d(1.0, xsi), py), d2m)
-    c4 = _edge_length(py[3], py[0], px[3], px[0], sph, np.einsum("ij,ji->i", _phi2d(eta, 0.0), py), d2m)
+    rows = trig.current().einsum_rows
+    c1 = _edge_length(py[0], py[1], px[0], px[1], sph, rows(_phi2d(0.0, xsi), py), d2m)
+    c2 = _edge_length(py[1], py[2], px[1], px[2], sph, rows(_phi2d(eta, 1.0), py), d2m)
+    c3 = _edge_length(py[2], py[3], px[2], px[3], sph, rows(_phi2d(1.0, xsi), py), d2m)
+    c4 = _edge_length(py[3], py[0], px[3], px[0], sph, rows(_phi2d(eta, 0.0), py), d2m)
     t_lv = (ti, np.clip(ti + 1, 0, tdim - 1)) if two_t else (ti,)
 
     def two_faces(data, zs, ys, xs):
@@ -361,7 +368,7 @@ def cgrid_velocity(fs, pos, gp):
         + (-eta * Uvel + (1 - xsi) * Vvel) * py[3]
     ) / jac
     if sph:
-        conv = d2m * np.cos(np.deg2rad(pos["y"]))
+        conv = d2m * trig.current().cgrid_conv(np.deg2rad(pos["y"]))
         u /= conv
         v /= conv
     if fs.W is not None:

@@ -437,7 +437,7 @@ def make_scalar_golden():
     np.savez_compressed(os.path.join(GOLDEN, "scalar_eval.npz"), **out)
 
 
-SCALAR_CURV_CASES = ("curv_sph_2d", "curv_flat_2d", "curv_sph_3d", "curv_sph_f32")
+SCALAR_CURV_CASES = ("curv_sph_2d", "curv_flat_2d", "curv_sph_3d", "curv_sph_f32", "curv_sph_dateline")
 
 
 def make_scalar_curv_golden(methods=("nearest", "cgrid_tracer"), out_name="scalar_eval_curv.npz"):

@@ -19,6 +19,8 @@ from __future__ import annotations
 
 import numpy as np
 
+from . import trig
+
 # --- status codes: _core/statuscodes.py:19-34 -------------------------------------------------
 SUCCESS, END_OF_LOOP, EVALUATE, REPEAT, DELETE = 0, 1, 10, 20, 30
 STOP_EXECUTION, STOP_ALL_EXECUTION = 40, 41
@@ -298,7 +300,7 @@ def xlinear_velocity(fs: OFieldSet, pos, gp):
     u = xlinear(fs.U, ti, tau, zi, zeta, yi, eta, xi, xsi)
     v = xlinear(fs.V, ti, tau, zi, zeta, yi, eta, xi, xsi)
     if fs.grid.spherical:
-        u /= fs.grid.deg2m * np.cos(np.deg2rad(pos["y"]))
+        u /= fs.grid.deg2m * trig.current().agrid_conv(np.deg2rad(pos["y"]))
         v /= fs.grid.deg2m
     if fs.W is not None:
         w = xlinear(fs.W, ti, tau, zi, zeta, yi, eta, xi, xsi)
@@ -354,7 +356,7 @@ def spatialslip_velocity(fs: OFieldSet, pos, gp, a, b):
     f_u[m] = f_u[m] * (1 - b * eta[m]) / (1 - eta[m])
     u = u * f_u
     if fs.grid.spherical:
-        u /= 1852 * 60 * np.cos(np.deg2rad(pos["y"]))
+        u /= 1852 * 60 * trig.current().agrid_conv(np.deg2rad(pos["y"]))
     f_v = np.ones_like(eta)
     m = all_land([(0, 0), (1, 0)]) & (xsi > 0)
     f_v[m] = f_v[m] * (a + b * xsi[m]) / xsi[m]
@@ -684,7 +686,7 @@ class DiffusionUniformKh:
         kh_zonal = eval_constant(fs, "Kh_zonal", p)
         kh_meridional = eval_constant(fs, "Kh_meridional", p)
         if fs.const_spherical:
-            kh_zonal = kh_zonal / pow(fs.const_deg2m * np.cos(p.y * np.pi / 180), 2)
+            kh_zonal = kh_zonal / pow(fs.const_deg2m * trig.current().kh_metric(p.y * np.pi / 180), 2)
             kh_meridional = kh_meridional / pow(fs.const_deg2m, 2)
         bx = np.sqrt(2 * kh_zonal)
         by = np.sqrt(2 * kh_meridional)
@@ -718,7 +720,7 @@ class _AdvectionDiffusion:
         sph, deg2m = fs.grid.spherical, fs.grid.deg2m
 
         def zonal(v, lat):  # meters_to_degrees_zonal (:11-13)
-            return v / pow(deg2m * np.cos(lat * np.pi / 180), 2)
+            return v / pow(deg2m * trig.current().m1em_metric(lat * np.pi / 180), 2)
 
         def merid(v):  # meters_to_degrees_meridional (:16-18)
             return v / pow(deg2m, 2)

@@ -100,6 +100,10 @@ __global__ void debug_math_kernel(int op, long long n, const double* a, const do
         case PB_MATH_DIV_BY_CACHED: o1 = 1.0 / b[i]; o0 = div_by_cached(x, b[i], o1); break;
         case PB_MATH_DIV_BY_CACHED_GUARDED: o1 = 1.0 / b[i]; o0 = div_by_cached_guarded(x, b[i], o1); break;
         case PB_MATH_BOX_MULLER_F32: box_muller_f32((uint32_t)x, (uint32_t)b[i], o0, o1); break;
+        case PB_MATH_COSF: o0 = (double)cosf_ool((float)x); break;
+        case PB_MATH_SINF: o0 = (double)sinf_ool((float)x); break;
+        case PB_MATH_COS: o0 = cos_ool(x); break;
+        case PB_MATH_SIN: o0 = sin_ool(x); break;
     }
     out[2 * i] = o0;
     out[2 * i + 1] = o1;

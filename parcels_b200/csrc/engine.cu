@@ -1567,8 +1567,8 @@ int32_t pb_debug_axis_cells(pb_engine* e, int32_t axis, int64_t cells, double* o
 
 int32_t pb_debug_math(pb_engine* e, int32_t op, int64_t n, const double* a, const double* b, double* out) {
     if (!e || n < 0 || (n && (!a || !out))) return fail(PB_ERR_INVALID, "NULL argument");
-    if (op < PB_MATH_COS_NP || op > PB_MATH_BOX_MULLER_F32) return fail(PB_ERR_INVALID, "unknown math op %d", op);
-    const bool binary = op >= PB_MATH_DIV_BY_CACHED;
+    if (op < PB_MATH_COS_NP || op > PB_MATH_SIN) return fail(PB_ERR_INVALID, "unknown math op %d", op);
+    const bool binary = op == PB_MATH_DIV_BY_CACHED || op == PB_MATH_DIV_BY_CACHED_GUARDED || op == PB_MATH_BOX_MULLER_F32;
     if (n && binary && !b) return fail(PB_ERR_INVALID, "math op %d needs a second operand", op);
     CK(cudaSetDevice(e->device));
     if (n == 0) return PB_OK;

@@ -432,7 +432,8 @@ class Engine:
         return out
 
     # pb_math_op (include/parcels_b200.h)
-    MATH_OPS = {"cos_np": 0, "sin_lat": 1, "sincos_lon": 2, "div_by_cached": 3, "div_by_cached_guarded": 4, "box_muller_f32": 5}
+    MATH_OPS = {"cos_np": 0, "sin_lat": 1, "sincos_lon": 2, "div_by_cached": 3, "div_by_cached_guarded": 4, "box_muller_f32": 5,
+                "cosf": 6, "sinf": 7, "cos": 8, "sin": 9}
 
     def debug_math(self, op, a, b=None):
         """The kernels' math primitive `op` evaluated on the device: (n, 2) float64 (see pb_debug_math)."""

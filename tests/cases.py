@@ -53,8 +53,9 @@ def smooth_uvw(rng, lon, lat, depth, nt, ddtype, umax=1.0, wmax=1e-3, noise=0.05
     return (umax * U).astype(ddtype), (umax * V).astype(ddtype), (wmax * W).astype(ddtype)
 
 
-def curv_mesh(ny, nx, spherical, cdtype):
-    """Smooth curvilinear node mesh (rotated 25 deg, stretched, warped): 2-D lon/lat (ny, nx)."""
+def curv_mesh(ny, nx, spherical, cdtype, sph_box=(-20.0, 30.0, 35.0, 25.0)):
+    """Smooth curvilinear node mesh (rotated 25 deg, stretched, warped): 2-D lon/lat (ny, nx).  Spherical meshes span
+    lon0 + dlon * X, lat0 + dlat * Y, sph_box = (lon0, dlon, lat0, dlat)."""
     I, J = np.meshgrid(np.linspace(0, 1, nx), np.linspace(0, 1, ny))
     th = np.deg2rad(25.0)
     a = I + 0.15 * I**2
@@ -62,7 +63,8 @@ def curv_mesh(ny, nx, spherical, cdtype):
     X = np.cos(th) * a - np.sin(th) * b
     Y = np.sin(th) * a + np.cos(th) * b
     if spherical:
-        lon, lat = -20 + 30 * X, 35 + 25 * Y
+        lon0, dlon, lat0, dlat = sph_box
+        lon, lat = lon0 + dlon * X, lat0 + dlat * Y
     else:
         # Warp BOTH grid-line families.  With straight, parallel eta-lines the quadratic coefficient of the
         # reference's bilinear inverse (index_search.py:136) cancels analytically to ~1e-10 -- above its
@@ -194,6 +196,25 @@ CASES = {
     "nearest_f32_static": dict(seed=35, kind="smooth", interp="nearest", cdtype="f4", ddtype="f4", mesh="flat", nx=9, ny=14, nz=3,
                                nt=1, tstep=1000.0, n=120, kernels=["AdvectionRK4_3D"], dt=600.0, segments=[dict(runtime=6000.0)],
                                delete=True, margin=0.1, umax=3.0),
+    # ---- spherical edge cases: where the trigonometry of the unit conversion and of the curvilinear search is at its worst ----
+    # within +-3 deg of the equator (nodes on it): cos_np's cancellation near 0 and its clamp to 1
+    "sph_equator": dict(seed=51, kind="smooth", cdtype="f8", ddtype="f4", mesh="spherical", nx=23, ny=25, nz=5, nt=3,
+                        tstep=3600.0, n=300, kernels=["AdvectionRK4_3D"], dt=600.0, segments=[dict(runtime=7200.0)],
+                        delete=True, margin=0.02, umax=2.0, lon_range=(-4.0, 4.0), lat_range=(-3.0, 3.0)),
+    # 80 - 89.5 deg: a small cos(lat) amplifies every last-bit difference of the zonal conversion; float32 coordinates and data
+    "sph_polar_f32": dict(seed=52, kind="smooth", cdtype="f4", ddtype="f4", mesh="spherical", nx=25, ny=20, nz=1, nt=3,
+                          tstep=3600.0, n=300, kernels=["AdvectionRK4"], dt=600.0, segments=[dict(runtime=7200.0)],
+                          delete=True, margin=0.02, umax=1.0, lon_range=(-30.0, 30.0), lat_range=(80.0, 89.5), no_depth=True),
+    # spherical rectilinear C-grid on float32 coordinates: at RK stage 1 the barycentric coordinates, the mid-edge latitudes and
+    # their cos are float32 (cgrid.cuh edge_length with L = float)
+    "cgrid_rect_sph_f32": dict(seed=53, kind="smooth", interp="cgrid_velocity", cdtype="f4", ddtype="f4", mesh="spherical",
+                               nx=21, ny=17, nz=5, nt=3, tstep=3600.0, n=300, kernels=["AdvectionRK4"], dt=600.0,
+                               segments=[dict(runtime=7200.0)], delete=True, margin=0.02, umax=10.0),
+    # curvilinear spherical C-grid across 90 deg, 135 deg and the antimeridian, longitudes wrapped to [-180, 180) like an ORCA
+    # grid: sincos_lon's quadrant switches, cos_np of |lon| > 90 deg (the cold path) and CGrid_Velocity's longitude unwrap
+    "curv_sph_dateline": dict(seed=54, kind="curv", cdtype="f8", mesh="spherical", nx=41, ny=25, nz=1, nt=3, tstep=7200.0,
+                              n=400, kernels=["AdvectionRK4"], dt=900.0, segments=[dict(runtime=14400.0)], delete=True,
+                              umax=20.0, sph_box=(95.0, 110.0, -10.0, 25.0), wrap_lon=True),
     "nearest_3d": dict(seed=33, kind="smooth", interp="nearest", cdtype="f8", ddtype="f4", mesh="spherical", nx=21, ny=17, nz=5,
                        nt=3, tstep=3600.0, n=300, kernels=["AdvectionRK4_3D"], dt=600.0, segments=[dict(runtime=7200.0)],
                        delete=True, margin=0.02, umax=10.0),
@@ -219,7 +240,7 @@ def build(spec):
     if spec["kind"] == "curv":
         cd = np.dtype(spec["cdtype"])
         nx, ny, nz, nt = spec["nx"], spec["ny"], spec["nz"], spec["nt"]
-        lon, lat = curv_mesh(ny, nx, mesh == "spherical", cd)
+        lon, lat = curv_mesh(ny, nx, mesh == "spherical", cd, **({"sph_box": spec["sph_box"]} if "sph_box" in spec else {}))
         three_d = spec["kernels"][0].endswith("_3D")
         depth = (np.linspace(0, 1, nz) ** 1.4 * 200.0).astype(cd) if nz > 1 else None
         shape = (nt, nz, ny, nx)
@@ -228,6 +249,9 @@ def build(spec):
         V = (umax * rng.uniform(-1, 1, shape)).astype(np.float32)
         W = (1e-2 * rng.uniform(-1, 1, shape)).astype(np.float32) if three_d else None
         x, y = points_in_mesh(rng, lon, lat, n)
+        if spec.get("wrap_lon"):  # nodes and releases wrapped to [-180, 180) after the releases were blended
+            lon = (((lon.astype(np.float64) + 180.0) % 360.0) - 180.0).astype(cd)
+            x = ((x + 180.0) % 360.0) - 180.0
         z = rng.uniform(2.0, 190.0, n) if nz > 1 else np.zeros(n)
         out.update(lon=lon, lat=lat, depth=depth, times=np.arange(nt) * spec["tstep"], U=U, V=V, W=W, x=x, y=y, z=z,
                    t=np.zeros(n), interp=spec.get("interp", "cgrid_velocity"), padding=("low", "low", "high"))  # fmt: skip
@@ -238,8 +262,8 @@ def build(spec):
     if "interp" in spec:
         out["interp"] = spec["interp"]
     if mesh == "spherical":
-        lon = np.linspace(-10.0, 10.0, nx).astype(cd)
-        lat = np.linspace(30.0, 50.0, ny).astype(cd)
+        lon = np.linspace(*spec.get("lon_range", (-10.0, 10.0)), nx).astype(cd)
+        lat = np.linspace(*spec.get("lat_range", (30.0, 50.0)), ny).astype(cd)
         umax = _default(spec, "umax", 1.0)
     else:
         lon = np.linspace(0.0, 2.0e4, nx).astype(cd)

@@ -6,23 +6,30 @@ while the particle was at |x| ~ 0.4 deg is 30 ulps of a final x = 0.02 deg (ever
 that ends next to zero; and with the oracle alone: perturbing its float32 cos by 1 ulp moves a particle
 ending at x = -0.0008 by 150 of ITS ulps).  The oracle itself is pinned to
 the reference's outputs with the reference's RNG (tests/test_advdiff_cpu.py).  Statistical check against the reference's
-own test (tests/test_diffusion.py:49-81): zero mean, zonal skew > meridional skew on a field with a zonal Kh gradient."""
+own test (tests/test_diffusion.py:49-81): zero mean, zonal skew > meridional skew on a field with a zonal Kh gradient.
+The spherical cases run once more against the oracle in engine arithmetic (``-exact`` ids: the device's cosf in the Kh metric and
+its cos in the unit conversion, tests/device_trig.py): positions bit-exact there too."""
 
 import numpy as np
 import pytest
 
 from advdiff_run import case_inputs, run_engine_advdiff, run_oracle_advdiff
+from device_trig import DeviceTrig
 from engine_run import ulp_diff_f32
+from oracle import trig
 from oracle.make_golden import ADVDIFF_CASES
 from philox_ref import device_normals, wiener_normals
 
 pytestmark = pytest.mark.gpu
 ERR_NAME = {60: "FieldOutOfBoundError", 61: "FieldOutOfBoundSurfaceError", 70: "OutsideTimeInterval", 51: "FieldInterpolationError"}
 FLAT = {"m1_flat", "em_f64_static", "em_raise", "m1_cgrid_flat"}
+ADVDIFF_MODES = [pytest.param(n, False, id=n) for n in ADVDIFF_CASES] + [
+    pytest.param(n, True, id=f"{n}-exact") for n in ADVDIFF_CASES if n not in FLAT
+]
 
 
-@pytest.mark.parametrize("name", list(ADVDIFF_CASES))
-def test_advdiff_matches_oracle_with_same_normals(name):
+@pytest.mark.parametrize("name, exact", ADVDIFF_MODES)
+def test_advdiff_matches_oracle_with_same_normals(name, exact):
     seed = 4242
     ps, err = run_engine_advdiff(name, seed=seed)
     state = {"it": 0}
@@ -32,14 +39,15 @@ def test_advdiff_matches_oracle_with_same_normals(name):
         state["it"] += 1
         return zx, zy
 
-    pd, oerr = run_oracle_advdiff(name, normal=normal)
+    with trig.use(DeviceTrig() if exact else trig.NumpyTrig()):
+        pd, oerr = run_oracle_advdiff(name, normal=normal)
     assert err == (ERR_NAME[oerr] if oerr else "")
     d = ps._data
     c0 = case_inputs(name)[0]
     for key in ("particle_id", "state", "t", "dt", "ei"):
         np.testing.assert_array_equal(d[key], pd[key], err_msg=f"{name}:{key}")
     for key in ("x", "y", "z"):
-        if name in FLAT:
+        if exact or name in FLAT:
             np.testing.assert_array_equal(d[key], pd[key], err_msg=f"{name}:{key}")
         else:
             start = np.asarray(c0[key], dtype=np.float64)[pd["particle_id"]]

@@ -11,7 +11,11 @@ cell indices and error states bit-exact; velocities
     float32, <= 64 float64 ulp otherwise (a lerp done in the wrong dtype is a 1e-8 relative error, 4e7 float64 ulp, and fails),
   * <= 64 float32 ulp on curvilinear meshes (hash hits carry float32-rounded (xsi, eta); the closed-form bilinear inverse
     amplifies last-ulp trig differences),
-all relative to the largest velocity of the batch (a sum of products has no better scale)."""
+all relative to the largest velocity of the batch (a sum of products has no better scale).
+
+In engine arithmetic (``-exact`` ids: the oracle's sin / cos are the device's own functions and waivers 4 and 8 take the engine's
+resolution, tests/device_trig.py) every case that has a tolerance above is compared bit for bit instead: float32 and float64
+positions, un-hinted and hinted."""
 
 import numpy as np
 import pytest
@@ -19,16 +23,28 @@ import pytest
 import cases
 from engine_run import make_fieldset
 from oracle import parcels_oracle as po
+from device_trig import DeviceTrig
+from oracle import trig
 from oracle_run import load_case, oracle_fieldset
 
 pytestmark = pytest.mark.gpu
 
 NAMES = ["c2_small", "flat_f32c_f64d", "all_f32", "c1_peninsula", "cgrid_rect_3d", "cgrid_rect_sph", "curv_flat_2d",
-         "curv_sph_2d", "curv_sph_3d", "curv_sph_f32", "curv_lin_flat_2d", "curv_lin_sph_3d", "curv_lin_sph_f32", "freeslip_3d", "partialslip_sph", "nearest_3d", "freeslip_surface"]  # fmt: skip
+         "curv_sph_2d", "curv_sph_3d", "curv_sph_f32", "curv_lin_flat_2d", "curv_lin_sph_3d", "curv_lin_sph_f32", "freeslip_3d", "partialslip_sph", "nearest_3d", "freeslip_surface",
+         "sph_equator", "sph_polar_f32", "cgrid_rect_sph_f32", "curv_sph_dateline"]  # fmt: skip
 
 
-def _assert_values(name, c, f32_positions, got, want, what):
+# the cases whose NumPy-trig comparison needs a tolerance get a second, bit-exact comparison in engine arithmetic
+EVAL_MODES = [pytest.param(n, False, id=n) for n in NAMES] + [
+    pytest.param(n, True, id=f"{n}-exact") for n in NAMES if n.startswith(("curv", "cgrid")) or cases.CASES[n]["mesh"] == "spherical"
+]
+
+
+def _assert_values(name, c, f32_positions, got, want, what, exact=False):
     want = np.asarray(want)
+    if exact:
+        np.testing.assert_array_equal(np.asarray(got, dtype=np.float64), want.astype(np.float64), err_msg=f"{name} {what}")
+        return
     scale = float(np.abs(want[np.isfinite(want)]).max()) if np.isfinite(want).any() else 0.0
     if name.startswith("curv"):
         tol = 64 * np.finfo(np.float32).eps
@@ -53,9 +69,14 @@ def _oracle_eval(ofs, t, z, y, x, three_d, hint):
     return out, pd["ei"][:, -1].copy(), pd["state"].copy()
 
 
-@pytest.mark.parametrize("name", NAMES)
+@pytest.mark.parametrize("name, exact", EVAL_MODES)
 @pytest.mark.parametrize("f32", [True, False])
-def test_single_eval_matches_oracle(name, f32):
+def test_single_eval_matches_oracle(name, exact, f32):
+    with trig.use(DeviceTrig() if exact else trig.NumpyTrig()):
+        _single_eval_vs_oracle(name, f32, exact)
+
+
+def _single_eval_vs_oracle(name, f32, exact):
     c = load_case(name)
     fs = make_fieldset(c)
     ofs = oracle_fieldset(c)
@@ -71,18 +92,18 @@ def test_single_eval_matches_oracle(name, f32):
                                           no_hint=True)  # fmt: skip
     np.testing.assert_array_equal(ei, oei)
     np.testing.assert_array_equal(st, ost)
-    _assert_values(name, c, f32, u, ou, "u")
-    _assert_values(name, c, f32, v, ov, "v")
+    _assert_values(name, c, f32, u, ou, "u", exact)
+    _assert_values(name, c, f32, v, ov, "v", exact)
     # second eval, slightly displaced, hinted with the cells just found
     x2 = (x + dt(0.01) * (x.max() - x.min()) / 30).astype(dt)
     (ou, ov, *ow), oei2, ost2 = _oracle_eval(ofs, t, z, y, x2, three_d, oei)
     u, v, w, ei2, st2 = eng.sample_velocity(t, z, y, x2, three_d=three_d, positions_are_f32=f32, ei_hint=oei)
     np.testing.assert_array_equal(ei2, oei2)
     np.testing.assert_array_equal(st2, ost2)
-    _assert_values(name, c, f32, u, ou, "u (hinted)")
-    _assert_values(name, c, f32, v, ov, "v (hinted)")
+    _assert_values(name, c, f32, u, ou, "u (hinted)", exact)
+    _assert_values(name, c, f32, v, ov, "v (hinted)", exact)
     if three_d:
-        _assert_values(name, c, f32, w, ow[0], "w (hinted)")
+        _assert_values(name, c, f32, w, ow[0], "w (hinted)", exact)
 
 
 @pytest.mark.parametrize("name", ["c2_small", "flat_f32c_f64d", "curv_sph_2d", "diffusion"])

@@ -8,7 +8,9 @@ import numpy as np
 import pytest
 
 import parcels_b200 as pb
+from device_trig import DeviceTrig
 from engine_run import ulp_diff_f32
+from oracle import trig
 from oracle_run import run_oracle
 
 pytestmark = pytest.mark.gpu
@@ -143,10 +145,16 @@ def test_fast_kernel_is_the_one_that_runs_and_refills_less_often_than_it_samples
     assert 0 < rep["cache_refills"] < rep["particle_steps"] // 4
 
 
-@pytest.mark.parametrize("mesh", ["spherical", "flat"])
-def test_fast_kernel_against_the_oracle(mesh):
+@pytest.mark.parametrize(
+    "mesh, schedule",
+    [pytest.param("spherical", None, id="spherical"), pytest.param("flat", None, id="flat")]
+    + [pytest.param("spherical", v, id=f"spherical-exact-schedule{v}") for v in (1, 2)],
+)
+def test_fast_kernel_against_the_oracle(mesh, schedule):
     """Directly against the CPU oracle (bit-exact ids / states / times / cells; positions bit-exact on the flat mesh, <= 2 float32
-    ulp on the spherical one, where CUDA's cos differs from libm's in the last place)."""
+    ulp on the spherical one, where CUDA's cos differs from libm's in the last place).  With a `schedule`, the spherical case
+    runs in that schedule of afast.cu against the oracle in engine arithmetic (the device's cosf / cos_np in the unit conversion,
+    tests/device_trig.py): positions bit-exact too, so the code afast.cu shares with the generic kernel is pinned by itself."""
     rng = np.random.default_rng(11)
     f = _field(rng, 24, 19, 7, 3, mesh, 3600.0, 3.0)
     n = 400
@@ -156,11 +164,27 @@ def test_fast_kernel_against_the_oracle(mesh):
              kernels=["AdvectionRK4_3D"], delete_on_error=True, dt=600.0, segments=[dict(runtime=7200.0)])  # fmt: skip
     from engine_run import run_engine
 
-    ps, err = run_engine(c)
-    pd, oerr = run_oracle(c)
+    if schedule is None:
+        ps, err = run_engine(c)
+        pd, oerr = run_oracle(c)
+    else:
+        os.environ["PB_DISABLE_FAST_KERNEL"] = "0"
+        os.environ["PB_FAST_KERNEL"] = str(schedule)
+        try:
+            ps, err = run_engine(c)
+        finally:
+            os.environ.pop("PB_DISABLE_FAST_KERNEL", None)
+            os.environ.pop("PB_FAST_KERNEL", None)
+        assert ps.last_report["kernel_variant"] == schedule
+        with trig.use(DeviceTrig()):
+            pd, oerr = run_oracle(c)
     assert err == "" and oerr is None
     d = ps._data
     for key in ("particle_id", "state", "t", "ei"):
         np.testing.assert_array_equal(d[key], pd[key], err_msg=key)
+    if schedule is not None:
+        for k in "xyz":
+            np.testing.assert_array_equal(d[k], pd[k], err_msg=k)
+        return
     worst = max(int(ulp_diff_f32(d[k], pd[k]).max()) for k in "xyz")
     assert worst <= (0 if mesh == "flat" else 2), worst

@@ -8,11 +8,12 @@ lenZ pre-pass all pass it.  This file checks those on the device:
 1. lane-order invariance at multi-block scale: the same set of particles (same ids, so the same Philox increments) in storage
    order, reversed and randomly permuted -- every column bit-identical per id, every launch report equal -- for every
    particle kernel family, plus a stratified subset (storage positions 0, 31, 32, B - 1, B, 3 B - 1, 3 B and N - 1 of both
-   orders; B = the launch block) against the oracle;
+   orders; B = the launch block) against the oracle -- within the trigonometry's tolerance against NumPy's sin / cos, and bit
+   for bit against the oracle evaluating the device's own (tests/device_trig.py);
 2. lane placement of the rare path: one particle that takes the side path (fast flow, released outside the domain, NaN,
    released later) in a set that never does -- and one hit-path particle among missing lanes -- at lanes 0, 1 and 31 of a
    warp, in the first and last warp of a block and in the first and last block: bit-identical wherever it sits, its
-   neighbours unchanged, and equal to the oracle;
+   neighbours unchanged, and equal to the oracle (bit for bit in engine arithmetic);
 3. warp-reduced reports against a recount from the returned arrays;
 4. the batch flags (`any(tau > 0)`, `any(zeta > 0)`) of pb_sample_velocity / pb_sample_scalar when the one sample that sets
    them sits at a lane / warp / block boundary of the pre-pass.
@@ -29,8 +30,10 @@ import pytest
 
 import cases
 import parcels_b200 as pb
+from device_trig import DeviceTrig
 from engine_run import ulp_diff_f32
 from oracle import parcels_oracle as po
+from oracle import trig
 from philox_ref import device_normals
 
 pytestmark = pytest.mark.gpu
@@ -240,6 +243,15 @@ def _oracle(c, ids):
 
 
 def _assert_oracle(c, got, ids, tol, what):
+    """Against the oracle with NumPy's trigonometry within `tol`; where tol > 0 (spherical or curvilinear), also against the
+    oracle in engine arithmetic (the device's own sin / cos, tests/device_trig.py) bit for bit."""
+    if tol:
+        with trig.use(DeviceTrig()):
+            _assert_oracle_within(c, got, ids, 0, what + " (engine arithmetic)")
+    return _assert_oracle_within(c, got, ids, tol, what)
+
+
+def _assert_oracle_within(c, got, ids, tol, what):
     pd, oerr = _oracle(c, ids)
     sel = np.isin(got["particle_id"], ids)
     mine = {k: v[sel] for k, v in got.items()}
@@ -405,6 +417,13 @@ def test_the_odd_particle_of_a_warp_is_the_same_wherever_it_sits(kernel, blocks)
 
 def _assert_oracle_ids(c, got, ids, tol, what):
     """_assert_oracle for a set whose inputs are given in `c` in the order of `ids` (arbitrary ids)."""
+    if tol:
+        with trig.use(DeviceTrig()):
+            _assert_oracle_ids_within(c, got, ids, 0, what + " (engine arithmetic)")
+    _assert_oracle_ids_within(c, got, ids, tol, what)
+
+
+def _assert_oracle_ids_within(c, got, ids, tol, what):
     pd, _ = _oracle_with_ids(c, ids)
     o = np.argsort(pd["particle_id"], kind="stable")
     g = np.argsort(got["particle_id"], kind="stable")

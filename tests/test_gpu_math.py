@@ -5,7 +5,15 @@ call), against a high-precision reference of the same operation.
   query vector;
 * sin_lat / sincos_lon (cgrid.cuh): the per-sample trigonometry of the curvilinear search;
 * div_by_cached / div_by_cached_guarded (common.cuh): division by a cached reciprocal (bcoords, the RK4 sum / 6, / deg2m);
-* box_muller_f32 (common.cuh): the float32 Box-Muller transform of DiffusionUniformKh's Wiener increments.
+* box_muller_f32 (common.cuh): the float32 Box-Muller transform of DiffusionUniformKh's Wiener increments;
+* cosf / sinf / cos / sin (cgrid.cuh cosf_ool, sinf_ool, cos_ool, sin_ool): CUDA's own functions, as the kernels call them (the
+  float32 unit conversions and hash queries, the per-cell table of the curvilinear search).  The oracle's engine-arithmetic mode
+  (tests/device_trig.py) evaluates its sin / cos through these ops, so each must be the function its name says: CUDA's documented
+  2 ulp of the exact value, float32 ulp for the float32 ops.
+  Limit: a bound cannot tell CUDA's cosf from a correctly rounded float64 cos rounded to float32 (both are float32 values within
+  2 float32 ulp), so a float32 op wired to (float)cos_ool would pass here.  That wiring is caught by the exact trajectory tests
+  instead: afast.cu's stage-1 cos done in float64 and rounded fails test_gpu_parity / test_gpu_fast_kernel's `-exact` cases on the
+  device.
 
 Error unit: ulp of the EXACT value y, 2^(floor(log2|y|) - 52) for float64 results (an exact zero must come out as zero).  The
 reference is np.longdouble (64-bit mantissa, asserted) for the dense sweeps and mpmath at 50 digits for the edge lists (long double
@@ -26,6 +34,7 @@ pytestmark = pytest.mark.gpu
 HOSTSIM = os.environ.get("PB_HOSTSIM_TEST") == "1"
 N = 2**16 if HOSTSIM else 2**24
 N_BM = 2**16 if HOSTSIM else 2**20
+N_F32 = 2**16 if HOSTSIM else 2**22
 
 try:
     import mpmath as _mpmath
@@ -240,6 +249,68 @@ def test_sincos_lon_cold_path_and_non_finite(eng):
     _check_sincos(eng, x, True, CUDA_TRIG_ULP, "cold path")
     nf = eng.debug_math("sincos_lon", np.array([np.inf, -np.inf, np.nan]))
     assert np.isnan(nf).all(), nf
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# CUDA's cosf / sinf / cos / sin, out of line as the kernels call them
+# ------------------------------------------------------------------------------------------------------------------------------
+def _f32_args(rng):
+    """float32 radians: uniform on [-4 pi, 4 pi], log-uniform magnitudes 2^-1 ... 2^-40, every half degree in [-720, 720] converted
+    like np.deg2rad of float32, and +-8 float32 neighbours of k pi/2 for |k| <= 16"""
+    f32 = np.float32
+    uni = rng.uniform(-4 * np.pi, 4 * np.pi, N_F32).astype(f32)
+    mag = (np.exp2(-rng.uniform(1.0, 40.0, N_F32)) * rng.choice([-1.0, 1.0], N_F32)).astype(f32)
+    deg = (np.arange(-1440, 1441) * 0.5).astype(f32) * f32(np.pi / 180.0)
+    mult = []
+    for k in range(-16, 17):
+        x = f32(k * (np.pi / 2))
+        lo = hi = x
+        mult.append(x)
+        for _ in range(8):
+            lo, hi = np.nextafter(lo, f32(-np.inf)), np.nextafter(hi, f32(np.inf))
+            mult += [lo, hi]
+    return np.concatenate([uni, mag, deg, np.array(mult, dtype=f32)])
+
+
+def _ulp_err_f32(dev, exact):
+    """|dev - exact| in float32 ulp of exact (long double arithmetic)"""
+    exact = np.asarray(exact, dtype=LD)
+    _, e = np.frexp(np.abs(exact))
+    ulp = np.ldexp(LD(1), e - 24)
+    return (np.abs(np.asarray(dev, dtype=LD) - exact) / ulp).astype(np.float64)
+
+
+@pytest.mark.parametrize("op, fn", [("cosf", np.cos), ("sinf", np.sin)])
+def test_cuda_float32_trig_error_bound(eng, op, fn):
+    assert _ld_ok()
+    x = _f32_args(np.random.default_rng(20261018))
+    out = eng.debug_math(op, x.astype(np.float64))[:, 0]
+    assert np.array_equal(out, out.astype(np.float32).astype(np.float64)), f"{op}: a result that is not a float32 value"
+    err = _ulp_err_f32(out, fn(x.astype(LD)))
+    assert err.max() <= CUDA_TRIG_ULP, f"{op}: {err.max():.3f} float32 ulp at x = {x[np.argmax(err)]!r}"
+    z = eng.debug_math(op, np.array([0.0, -0.0]))[:, 0]
+    assert np.array_equal(z, [1.0, 1.0] if op == "cosf" else [0.0, -0.0]) and (op == "cosf" or np.signbit(z[1]))
+    assert np.isnan(eng.debug_math(op, np.array([np.inf, -np.inf, np.nan]))[:, 0]).all()
+
+
+def test_cuda_float32_trig_rounds_its_argument_to_float32(eng):
+    """The float32 ops see the float32 value carried in the double slot: a float64 argument is rounded first."""
+    x = np.array([0.1, 1.0 + 2.0**-40, 2.5], dtype=np.float64)
+    for op in ("cosf", "sinf"):
+        np.testing.assert_array_equal(eng.debug_math(op, x)[:, 0], eng.debug_math(op, x.astype(np.float32).astype(np.float64))[:, 0])
+
+
+@pytest.mark.parametrize("op, fn_ld, fn_mp", [("cos", np.cos, "cos"), ("sin", np.sin, "sin")])
+def test_cuda_float64_trig_error_bound(eng, op, fn_ld, fn_mp):
+    rng = np.random.default_rng(20261019)
+    fmp = getattr(MP, fn_mp) if MP else None
+    uni = rng.uniform(-4 * np.pi, 4 * np.pi, N)
+    err = _ulp_err(eng.debug_math(op, uni)[:, 0], uni, fn_ld, fmp, False)
+    assert err.max() <= CUDA_TRIG_ULP, f"{op} uniform: {err.max():.3f} ulp at x = {uni[np.argmax(err)]!r}"
+    edge = np.concatenate([_lon_edge(), _latitudes_edge(), [20.0, 100.0, 1e4, -1e9]])
+    err = _ulp_err(eng.debug_math(op, edge)[:, 0], edge, fn_ld, fmp, True)
+    assert err.max() <= CUDA_TRIG_ULP, f"{op} edges: {err.max():.3f} ulp at x = {edge[np.argmax(err)]!r}"
+    assert np.isnan(eng.debug_math(op, np.array([np.inf, -np.inf, np.nan]))[:, 0]).all()
 
 
 # ------------------------------------------------------------------------------------------------------------------------------

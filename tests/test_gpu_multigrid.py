@@ -7,7 +7,9 @@ import numpy as np
 import pytest
 
 import parcels_b200 as pb
+from device_trig import DeviceTrig
 from oracle import parcels_oracle as po
+from oracle import trig
 from parcels_b200.fieldset import XGrid
 
 pytestmark = pytest.mark.gpu
@@ -42,8 +44,11 @@ def _setup(curvilinear_second):
     return fs, ofs1, ofs2, wind, (x, y, z), times
 
 
-@pytest.mark.parametrize("curv", [False, True])
-def test_field_on_a_second_grid_samples_like_the_oracle(curv):
+@pytest.mark.parametrize("curv, exact", [pytest.param(False, False, id="False"), pytest.param(True, False, id="True"),
+                                         pytest.param(True, True, id="True-exact")])  # fmt: skip
+def test_field_on_a_second_grid_samples_like_the_oracle(curv, exact):
+    """`exact`: the curvilinear second grid against the oracle in engine arithmetic (the scalar sampler's trigonometry,
+    tests/device_trig.py): values bit-exact instead of within 64 float32 ulp."""
     fs, ofs1, ofs2, wind, (x, y, z), times = _setup(curv)
     assert len(fs.gridset) == 2
     ps = pb.ParticleSet(fs, x=x, y=y, z=z, t=np.zeros(len(x)))
@@ -52,10 +57,11 @@ def test_field_on_a_second_grid_samples_like_the_oracle(curv):
     v = fs.wind.eval(tq, ps._data["z"], ps._data["y"], ps._data["x"], ps)
     pd = po.create_particle_data(x, y, z, np.zeros(len(x)), ngrids=2)
     view = po.View(pd, np.ones(len(x), dtype=bool))
-    ov = po.eval_scalar(ofs2, wind, "linear", tq, pd["z"], pd["y"], pd["x"], view)
+    with trig.use(DeviceTrig(scalar_sampler=True) if exact else trig.NumpyTrig()):
+        ov = po.eval_scalar(ofs2, wind, "linear", tq, pd["z"], pd["y"], pd["x"], view)
     np.testing.assert_array_equal(ps._data["ei"][:, -1], pd["ei"][:, -1])
     np.testing.assert_array_equal(ps._data["state"], pd["state"])
-    if curv:
+    if curv and not exact:
         np.testing.assert_allclose(v, ov, rtol=0, atol=64 * np.finfo(np.float32).eps * 5.0)
     else:
         np.testing.assert_array_equal(v, ov)

@@ -9,6 +9,9 @@ Bar (stated tolerance):
   reference's order and dtype with FMA contraction off); on spherical meshes <= 2 float32 ulp
   (``cos`` of CUDA libdevice vs glibc/NumPy is not bit-identical); on curvilinear meshes <= 8 float32
   ulp (see CURV_ULP).
+* Engine arithmetic (``-exact`` ids): every spherical and curvilinear case once more against the oracle evaluating its sin / cos
+  with the device's own functions and the engine's resolution of waivers 4 and 8 (tests/device_trig.py): x, y, z bit-exact too.
+  The tolerances above are then only the trigonometry's, and an arithmetic slip that moves a position by one ulp fails here.
 """
 
 import os
@@ -20,6 +23,8 @@ import cases
 from engine_run import make_fieldset, run_engine, ulp_diff_f32
 from oracle import parcels_oracle as po
 from oracle_run import load_case, run_oracle
+from device_trig import DeviceTrig
+from oracle import trig
 from philox_ref import device_normals, wiener_normals
 
 pytestmark = pytest.mark.gpu
@@ -32,7 +37,24 @@ FLAT_EXACT = {"flat_f32c_f64d", "c1_peninsula", "delayed_partial", "raise_oob", 
 # BLAS summation order, libm vs libdevice trig) by the cell's condition number, and spatial-hash hits are
 # rounded to float32 (spatialhash.py:511) -- a flipped rounding moves a weight by 6e-8.  Stated tolerance:
 CURV_ULP = 8
+# A spherical C-grid on float32 coordinates evaluates its first RK stage in float32 throughout: four edge lengths, each through the
+# float32 cos of a float32 mid-edge latitude, and the conversion's cosf -- CUDA's cosf (<= 2 ulp) against NumPy's float32 cos
+# there moved y by 3 float32 ulp on an H100.  Its `-exact` comparison (the device's own cosf in the oracle) is bit-exact.
+F32_CGRID_SPH_ULP = {"cgrid_rect_sph_f32": 4}
 NON_DIFFUSION = [n for n in cases.CASES if "DiffusionUniformKh" not in cases.CASES[n]["kernels"]]
+# every case once against the NumPy-trig oracle (the reference's values), the spherical and curvilinear ones once more in
+# engine arithmetic
+ORACLE_MODES = [pytest.param(n, False, id=n) for n in NON_DIFFUSION] + [
+    pytest.param(n, True, id=f"{n}-exact") for n in NON_DIFFUSION if n not in FLAT_EXACT
+]
+
+
+def oracle_in_mode(c, exact, **kw):
+    """run_oracle with the NumPy trigonometry of the reference, or (exact) in engine arithmetic."""
+    if not exact:
+        return run_oracle(c, **kw)
+    with trig.use(DeviceTrig()):
+        return run_oracle(c, **kw)
 
 
 def _compare(name, d, ref, exact_xyz):
@@ -44,15 +66,15 @@ def _compare(name, d, ref, exact_xyz):
             np.testing.assert_array_equal(d[key], ref[key], err_msg=f"{name}:{key}")
         else:
             ulps = ulp_diff_f32(d[key], ref[key])
-            tol = CURV_ULP if name.startswith("curv") else 2
+            tol = CURV_ULP if name.startswith("curv") else F32_CGRID_SPH_ULP.get(name, 2)
             assert ulps.max() <= tol, f"{name}:{key} differs by {ulps.max()} f32 ulp"
 
 
-@pytest.mark.parametrize("name", NON_DIFFUSION)
-def test_engine_matches_oracle(name):
+@pytest.mark.parametrize("name, exact", ORACLE_MODES)
+def test_engine_matches_oracle(name, exact):
     c = load_case(name)
     ps, err = run_engine(c)
-    pd, oerr = run_oracle(c)
+    pd, oerr = oracle_in_mode(c, exact)
     assert err == (ERR_NAME[oerr] if oerr else "")
     if name == "raise_time":
         # whole-view OutsideTimeInterval: states/positions/time pinned; dx/ei of the aborted step waived
@@ -60,7 +82,7 @@ def test_engine_matches_oracle(name):
         for key in ("x", "y", "z", "t"):
             np.testing.assert_array_equal(ps._data[key], pd[key])
         return
-    _compare(name, ps._data, pd, name in FLAT_EXACT)
+    _compare(name, ps._data, pd, exact or name in FLAT_EXACT)
 
 
 @pytest.mark.parametrize("name", NON_DIFFUSION)
@@ -124,6 +146,15 @@ def test_device_philox_matches_numpy_restatement():
 def test_fused_diffusion_matches_oracle_with_same_normals():
     """DiffusionUniformKh: deterministic part compared with the oracle fed the engine's Philox
     stream; statistical parity with the reference's RNG is covered in test_gpu_properties."""
+    _fused_diffusion_vs_oracle(exact=False)
+
+
+def test_fused_diffusion_matches_oracle_in_engine_arithmetic():
+    """The same with the device's cos in the oracle (unit conversion and Kh metric): positions bit-exact."""
+    _fused_diffusion_vs_oracle(exact=True)
+
+
+def _fused_diffusion_vs_oracle(exact):
     c = load_case("diffusion")
     seed = 99
     ps, err = run_engine(c, seed=seed)
@@ -139,11 +170,14 @@ def test_fused_diffusion_matches_oracle_with_same_normals():
         calls["n"] += 1
         return zx, zy
 
-    pd, oerr = run_oracle(c, normal=normal)
+    pd, oerr = oracle_in_mode(c, exact, normal=normal)
     assert oerr is None and calls["n"] > 0
     np.testing.assert_array_equal(ps._data["particle_id"], pd["particle_id"])
     np.testing.assert_array_equal(ps._data["state"], pd["state"])
     np.testing.assert_array_equal(ps._data["ei"], pd["ei"])
     for key in ("x", "y", "z"):
-        ulps = ulp_diff_f32(ps._data[key], pd[key])
-        assert ulps.max() <= 4, f"{key}: {ulps.max()} ulp"
+        if exact:
+            np.testing.assert_array_equal(ps._data[key], pd[key], err_msg=key)
+        else:
+            ulps = ulp_diff_f32(ps._data[key], pd[key])
+            assert ulps.max() <= 4, f"{key}: {ulps.max()} ulp"

@@ -1,15 +1,20 @@
 """GPU parity of AdvectionRK45 (pb_advect_rk45: the Repeat / next_dt state machine in one device kernel) against the
 oracle and against the reference's own outputs (tests/golden/rk45.npz): positions bit-exact on flat meshes and <= 2
 float32 ulp on spherical ones; times, per-particle dt and next_dt, states and cell indices bit-exact; the number of
-RK45 attempts (accepted + rejected) equal to the oracle's."""
+RK45 attempts (accepted + rejected) equal to the oracle's.  In engine arithmetic (``-exact`` ids: the oracle's sin / cos are the
+device's own functions, tests/device_trig.py) the spherical and curvilinear cases are bit-exact as well, with the same number of
+attempts and no particle left out of the comparison."""
 
 import os
 
 import numpy as np
 import pytest
 
+import cases
 import parcels_b200 as pb
+from device_trig import DeviceTrig
 from oracle import parcels_oracle as po
+from oracle import trig
 from engine_run import make_fieldset, ulp_diff_f32
 from oracle.make_golden import RK45_CASES
 from oracle_run import load_case, oracle_fieldset
@@ -19,10 +24,20 @@ pytestmark = pytest.mark.gpu
 NEXT_DT = pb.Particle.add_variable(pb.Variable("next_dt", dtype=np.float32, initial=0))
 
 
-def _engine_rk45(name, kernels=None):
+def _flat_rectilinear(name):
+    return cases.CASES[name]["mesh"] == "flat" and not name.startswith("curv")
+
+
+RK45_MODES = [pytest.param(n, False, id=n) for n in RK45_CASES] + [
+    pytest.param(n, True, id=f"{n}-exact") for n in RK45_CASES if not _flat_rectilinear(n)
+]
+
+
+def _engine_rk45(name, kernels=None, exact=False):
     tol, min_dt, fmax, runtime, dt = RK45_CASES[name]
     attempts = [0]
-    c, pd, steps, _ = run_oracle_rk45(name, attempts)
+    with trig.use(DeviceTrig() if exact else trig.NumpyTrig()):
+        c, pd, steps, _ = run_oracle_rk45(name, attempts)
     c = dict(c, W=None)
     fs = make_fieldset(c)
     fs.add_context("RK45_tol", tol)  # metres: converted to degrees when the kernel list is built, like the reference
@@ -33,14 +48,19 @@ def _engine_rk45(name, kernels=None):
     return c, ps, pd, steps, attempts[0]
 
 
-@pytest.mark.parametrize("name", list(RK45_CASES))
-def test_rk45_matches_oracle_and_reference(name, golden_dir):
+@pytest.mark.parametrize("name, engine_arithmetic", RK45_MODES)
+def test_rk45_matches_oracle_and_reference(name, engine_arithmetic, golden_dir):
     g = np.load(os.path.join(golden_dir, "rk45.npz"))
-    c, ps, pd, steps, attempts = _engine_rk45(name)
+    c, ps, pd, steps, attempts = _engine_rk45(name, exact=engine_arithmetic)
     d = ps._data
     assert ps.last_report["particle_steps"] == steps
     curv = name.startswith("curv")
-    exact = c["mesh"] == "flat" and not curv
+    if engine_arithmetic:
+        for k in ("x", "y", "z", "t", "dt", "next_dt", "state", "ei"):
+            np.testing.assert_array_equal(d[k], pd[k], err_msg=f"{name}:{k}")
+        assert ps.last_report["cache_refills"] == 6 * attempts  # field evaluations: same accept / reject sequence
+        return
+    exact = _flat_rectilinear(name)
     for ref in (pd, {k: g[f"{name}/{k}"] for k in ("x", "y", "z", "t", "dt", "next_dt", "state", "ei")}):
         for k in ("state", "z") + (() if curv else ("ei",)):
             np.testing.assert_array_equal(d[k], ref[k], err_msg=f"{name}:{k}")

@@ -12,6 +12,8 @@ from engine_run import make_fieldset
 from oracle import parcels_oracle as po
 from oracle.make_golden import SCALAR_CASES, land_tracer_inputs, scalar_inputs
 from oracle_run import load_case, oracle_fieldset
+from device_trig import DeviceTrig
+from oracle import trig
 
 pytestmark = pytest.mark.gpu
 
@@ -101,7 +103,7 @@ def test_user_sampling_kernel_in_a_mixed_list():
     assert np.abs(ps._data["p"]).max() > 0
 
 
-@pytest.mark.parametrize("name", ["curv_sph_2d", "curv_flat_2d", "curv_sph_3d", "curv_sph_f32"])
+@pytest.mark.parametrize("name", ["curv_sph_2d", "curv_flat_2d", "curv_sph_3d", "curv_sph_f32", "curv_sph_dateline"])
 def test_scalar_eval_on_curvilinear_grids(name, golden_dir):
     """CGrid_Tracer / XNearest on curvilinear C-grids (NEMO tracers on an ORCA grid): a fresh set -- the whole batch through the
     spatial hash, like the reference -- and a displaced float64 evaluation hinted by the cells just found; values, cells and
@@ -130,13 +132,18 @@ def test_scalar_eval_on_curvilinear_grids(name, golden_dir):
         make_fieldset(c).add_field("Q", P, interp_method="linear_invdist_land")
 
 
-@pytest.mark.parametrize("name", ["curv_sph_2d", "curv_flat_2d", "curv_sph_3d", "curv_sph_f32"])
-def test_xlinear_scalar_eval_on_curvilinear_grids(name, golden_dir):
+CURV_SCALAR = ["curv_sph_2d", "curv_flat_2d", "curv_sph_3d", "curv_sph_f32", "curv_sph_dateline"]
+
+
+@pytest.mark.parametrize("name, exact", [pytest.param(n, False, id=n) for n in CURV_SCALAR] + [pytest.param(n, True, id=f"{n}-exact") for n in CURV_SCALAR])
+def test_xlinear_scalar_eval_on_curvilinear_grids(name, exact, golden_dir):
     """XLinear behind the curvilinear search (an A-grid tracer on 2-D lon / lat), against the reference's own values
     (tests/golden/scalar_eval_curv_linear.npz): cells and states bit-exact; values within 64 float32 ulp of the field's range --
     the barycentric coordinates come out of the closed-form bilinear inverse (last-ulp trig differences amplified, hash hits
     rounded to float32: the curvilinear tolerance of the trajectory tests), and the reference's float32-TYPED coordinates after
-    a hash hit (DESIGN.md waiver 4) are float32-rounded float64 values here, so the value is always float64."""
+    a hash hit (DESIGN.md waiver 4) are float32-rounded float64 values here, so the value is always float64.  `exact`: the values
+    are compared bit for bit with the oracle in engine arithmetic instead (the scalar sampler's own trigonometry and waiver 4's
+    resolution, tests/device_trig.py)."""
     g = np.load(os.path.join(golden_dir, "scalar_eval_curv_linear.npz"))
     c = load_case(name)
     for T in (c["U"].shape[0], 1):
@@ -153,6 +160,19 @@ def test_xlinear_scalar_eval_on_curvilinear_grids(name, golden_dir):
         np.testing.assert_array_equal(ei1, g[f"{key}/ei"], err_msg=key)
         np.testing.assert_array_equal(ps._data["ei"], g[f"{key}/ei2"], err_msg=key + " second")
         np.testing.assert_array_equal(ps._data["state"], g[f"{key}/state2"], err_msg=key + " second")
+        if exact:
+            ofs = oracle_fieldset(c)
+            pd = po.create_particle_data(c["x"], c["y"], c["z"], c["t"], ngrids=ofs.ngrids)
+            view = po.View(pd, np.ones(len(pd["x"]), dtype=bool))
+            with trig.use(DeviceTrig(scalar_sampler=True)):
+                o1 = po.eval_scalar(ofs, P, "linear", tq, pd["z"], pd["y"], pd["x"], view)
+                np.testing.assert_array_equal(ei1, pd["ei"], err_msg=key)
+                o2 = po.eval_scalar(ofs, P, "linear", tq, pd["z"], np.asarray(pd["y"], dtype=np.float64), x2, view)
+            np.testing.assert_array_equal(ps._data["ei"], pd["ei"], err_msg=key + " second")
+            np.testing.assert_array_equal(ps._data["state"], pd["state"], err_msg=key + " second")
+            np.testing.assert_array_equal(v1, o1, err_msg=key)
+            np.testing.assert_array_equal(v2, o2, err_msg=key + " second")
+            continue
         np.testing.assert_allclose(v1, g[f"{key}/value"].astype(np.float64), rtol=0, atol=tol, err_msg=key)
         np.testing.assert_allclose(v2, g[f"{key}/value2"].astype(np.float64), rtol=0, atol=tol, err_msg=key + " second")
         assert np.abs(g[f"{key}/value"]).max() > 0
