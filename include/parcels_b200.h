@@ -311,7 +311,8 @@ typedef struct pb_rk45_args {
 int32_t pb_advect_rk45(pb_engine* e, const pb_rk45_args* args, double* dt_inout, double* next_dt_inout, pb_report* rep);
 /* The same loop on the RESIDENT dt / next_dt / iteration columns of pb_particles_upload_resume (read them back with
  * pb_particles_download_resume): the route of a domain-decomposed engine (mode D, below), where these travel with the particles,
- * and the one RK45 entry point that runs there (rectilinear A-grid, XLinear_Velocity).  kernels_only must be 0.  A particle that
+ * and the one RK45 entry point that runs there (rectilinear grids: XLinear_Velocity, XFreeslip, XPartialslip, CGrid_Velocity).
+ * kernels_only must be 0.  A particle that
  * leaves the owned slab stops mid-call with its dt, next_dt and iteration count, and the launch with resume = 1 on its new owner
  * continues it.  Without waiting (pb_last_report collects the report); no batch-level clamp of the particles that left the loop
  * early: pb_rk45_finalize_resident does it once the whole call is done, with the call's iteration count over all launches and
@@ -388,7 +389,7 @@ int32_t pb_sample_scalar(pb_engine* e, int32_t slot, int32_t method, int64_t n, 
  * bounds[nranks+1]: rank r advances particles with bounds[r] <= x < bounds[r+1] (rank 0 also everything left
  * of bounds[1], the last rank everything right of bounds[nranks-1]); pb_advect stops a particle as soon as
  * it leaves the owned interval (pb_report.n_migrate).  A stage position outside owned+halo columns is a
- * halo violation: state 99, counted in n_error.
+ * halo violation: state 99, counted in n_error (the DeleteParticle handler leaves it alone, so pb_report.max_state shows it).
  * Migration round: pb_migrate_count -> (exchange counts) -> pb_migrate_pack -> all-to-all-v of the 48-byte
  * records over NCCL -> pb_migrate_unpack (compacts the stayers, appends the arrivals) -> pb_advect(resume=1). */
 int32_t pb_decomp_set(pb_engine* e, int32_t nranks, int32_t rank, const double* bounds, int64_t xi_offset,

@@ -455,9 +455,19 @@ struct CGridPolicy {
             const TY eta = axis_search<PY, A>((const A*)g.lat, g.ny, y, e.cy);
             const TX xsi = axis_search<PX, A>((const A*)g.lon, g.nx, x, e.cx);
             yi = e.cy.idx; xi = e.cx.idx;
-            long long r = (long long)yi * g.xdim + (long long)xi;
+            // mode D: ei is raveled from the global column.  A sentinel at a slab edge that is not the edge of the global domain
+            // means the position left the owned + halo columns (the halo is too small for this dt): state 99, no value.  Inside
+            // the slab the face reads xi + off_x and xi + 1 stay within the slab's columns (halo >= 1), so load_faces' clamps act
+            // only at global edges, as on one GPU.
+            const int gxi = (g.decomposed && xi >= 0) ? xi + g.xi_offset : xi;
+            long long r = (long long)yi * g.xdim + (long long)gxi;
             if (g.nz > 0) r += (long long)zi * (g.ydim * g.xdim);
             e.ei = (int)r;
+            if (g.decomposed && ((xi == -2 && !g.left_global) || (xi == -1 && !g.right_global))) {
+                e.state = max(e.state, 99);
+                u = Val{0.0, false}; v = u; w = u;
+                return;
+            }
             int s = e.state;
             if (xi == -1 || yi == -1 || zi == -1) s = max(s, (int)PB_ERROR_OUT_OF_BOUNDS);
             if (zi == -2) s = max(s, (int)PB_ERROR_THROUGH_SURFACE);

@@ -1429,8 +1429,11 @@ int32_t pb_advect_rk45_resident_async(pb_engine* e, const pb_rk45_args* a) {
     if (!e->resume_on) return fail(PB_ERR_STATE, "dt / next_dt / iteration columns not resident (pb_particles_upload_resume)");
     int32_t rc = check_fields(e, 2);
     if (rc) return rc;
-    if (e->interp != PB_INTERP_XLINEAR_VELOCITY || e->g.curvilinear)
-        return fail(PB_ERR_INVALID, "pb_advect_rk45_resident runs on rectilinear A-grids with XLinear_Velocity");
+    const bool cgrid = e->interp == PB_INTERP_CGRID_VELOCITY;
+    const bool slip = agrid_alt_mode(e->interp) == 1;
+    if (!(cgrid || e->interp == PB_INTERP_XLINEAR_VELOCITY || slip) || e->g.curvilinear)
+        return fail(PB_ERR_INVALID, "pb_advect_rk45_resident runs on rectilinear grids with XLinear_Velocity, XFreeslip, XPartialslip "
+                                    "or CGrid_Velocity");
     CK(cudaSetDevice(e->device));
     AdvectParams p{};
     fill_advect_params(e, a, p);
@@ -1440,8 +1443,12 @@ int32_t pb_advect_rk45_resident_async(pb_engine* e, const pb_rk45_args* a) {
     if ((rc = begin_launch(e))) return rc;
     if (e->n > 0) {
         const ResumeDev r = e->cur.resume();
-        cudaError_t ce = launch_rk45(p, r.dt, r.next_dt, r.iters, a->next_dt_is_f32, a->tol, a->min_dt, a->max_dt, e->coord_f64 != 0,
-                                     e->f_f64[0] != 0, e->g.nt > 0, e->stream);
+        cudaError_t ce = cgrid ? launch_rk45_cgrid(p, r.dt, r.next_dt, r.iters, a->next_dt_is_f32, a->tol, a->min_dt, a->max_dt,
+                                                   e->coord_f64 != 0, e->f_f64[0] != 0, e->stream)
+                         : slip ? launch_rk45_slip(p, r.dt, r.next_dt, r.iters, a->next_dt_is_f32, a->tol, a->min_dt, a->max_dt,
+                                                  e->coord_f64 != 0, e->f_f64[0] != 0, e->g.nt > 0, e->stream)
+                                : launch_rk45(p, r.dt, r.next_dt, r.iters, a->next_dt_is_f32, a->tol, a->min_dt, a->max_dt,
+                                              e->coord_f64 != 0, e->f_f64[0] != 0, e->g.nt > 0, e->stream);
         if (ce != cudaSuccess) return fail(PB_ERR_CUDA, "rk45_kernel launch failed: %s", cudaGetErrorString(ce));
     }
     return end_launch(e);
@@ -1476,9 +1483,9 @@ int32_t pb_advect_diffusion_async(pb_engine* e, const pb_advdiff_args* a) {
     if ((e->interp != PB_INTERP_XLINEAR_VELOCITY && e->interp != PB_INTERP_CGRID_VELOCITY) || e->g.curvilinear)
         return fail(PB_ERR_INVALID, "AdvectionDiffusionM1/EM run on rectilinear fields with XLinear_Velocity or CGrid_Velocity");
     // under domain decomposition every lane's iteration count travels with its particle: a resident column
-    if (e->g.decomposed && (e->interp != PB_INTERP_XLINEAR_VELOCITY || !e->resume_on))
-        return fail(PB_ERR_INVALID, "AdvectionDiffusionM1/EM under domain decomposition run with XLinear_Velocity on the resident "
-                                    "iteration columns (pb_particles_upload_resume)");
+    if (e->g.decomposed && !e->resume_on)
+        return fail(PB_ERR_INVALID, "AdvectionDiffusionM1/EM under domain decomposition run on the resident iteration columns "
+                                    "(pb_particles_upload_resume)");
     if (!e->have_pid) return fail(PB_ERR_STATE, "diffusion needs particle_id (RNG counter)");
     FieldDev fkz, fkm;
     if ((rc = scalar_field_desc(e, a->kh_zonal_slot, fkz))) return rc;

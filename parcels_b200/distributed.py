@@ -128,12 +128,17 @@ class _SlabLevels:
 
 
 class DecomposedFieldSet:
-    """This rank's X-slab of a rectilinear A-grid FieldSet, resident on ``device`` (``time_window=W``: only W time levels of it)."""
+    """This rank's X-slab of a rectilinear FieldSet, resident on ``device`` (``time_window=W``: only W time levels of it).
+    ``interp_method`` and ``padding`` are those of ``FieldSet.from_arrays``: an A-grid with XLinear_Velocity ("linear"), XFreeslip,
+    XPartialslip or nearest-node sampling, or a C-grid with CGrid_Velocity and its SGRID padding."""
 
     def __init__(self, *, lon, lat, U, V, W=None, depth=None, time=None, mesh="spherical", rank, world, halo_cells=4,
-                 device=0, time_window=None):  # fmt: skip
+                 device=0, time_window=None, interp_method="linear", padding=("low", "low", "high")):  # fmt: skip
         from .fieldset import FieldSet
 
+        if np.ndim(lon) != 1 or np.ndim(lat) != 1:
+            raise NotImplementedError("domain decomposition cuts rectilinear grids (1-D lon / lat) into longitude slabs; on a "
+                                      "curvilinear grid a slab is not a range of longitudes")  # fmt: skip
         self.rank, self.world, self.device = rank, world, device
         self.plan = slab_plan(lon, world, halo_cells)[rank]
         lo, hi = self.plan["lo"], self.plan["hi"]
@@ -144,6 +149,7 @@ class DecomposedFieldSet:
             cut = lambda a: _SlabLevels(a, sl)  # noqa: E731
         self.fs = FieldSet.from_arrays(lon=np.ascontiguousarray(np.asarray(lon)[sl]), lat=lat, depth=depth, time=time,
                                        U=cut(U), V=cut(V), W=None if W is None else cut(W), mesh=mesh, time_window=time_window,
+                                       interp_method=interp_method, padding=padding,
                                        xdim=np.asarray(lon).size - 1)  # fmt: skip  (GLOBAL cell count: ei stays global)
         self._attach()
 
@@ -292,8 +298,12 @@ def _advect_args(eng, plan, dt, endtime, first, seed, rng_call, rounds):
     # migration round is a new launch on every rank (the round count is global), so the round number joins the call index and no
     # particle ever draws the same increment twice, wherever it migrates.  (The stream differs from a single-GPU run's, whose
     # iterations are not cut into rounds: statistically equivalent, not bit-identical -- the advection-only path is.)
+    # The fixed-step kernel restarts its iteration count in every launch, so the first-evaluation time bit reaches the first
+    # iteration of every round.  That is the single-GPU rule: the bit changes a value only on the first time level (tau == 0), where
+    # a particle is before its first step -- a lane the first round only routed to its owner, or one that waited for the window.
     return eng.make_args(plan.scheme, dt, endtime, delete_on_error=True, resume=not first, diffusion=plan.diffusion, kh=plan.kh,
-                         kh_spherical=plan.kh_spherical, kh_deg2m=plan.kh_deg2m, seed=seed, rng_call=(int(rng_call) << 20) + rounds)  # fmt: skip
+                         kh_spherical=plan.kh_spherical, kh_deg2m=plan.kh_deg2m, seed=seed, rng_call=(int(rng_call) << 20) + rounds,
+                         batch_levels=plan.batch_levels)  # fmt: skip
 
 
 def _advect_round(dfs, args, sign):
@@ -427,7 +437,7 @@ def decomposed_plan(dfs: DecomposedFieldSet, kernels, pdata: dict | None = None)
     if not plan.delete_on_error:
         raise NotImplementedError("domain-decomposed execution needs the DeleteParticle handler (errors cannot be replayed "
                                   "step-exactly across ranks)")  # fmt: skip
-    plan.batch_levels = 0  # the call's batch-level bits (execute_decomposed sets them for the kernels that carry their iterations)
+    plan.batch_levels = 0  # the call's batch-level bits (execute_decomposed sets them, except for fixed-step XLinear_Velocity lists)
     plan.next_dt_dtype = np.dtype(pdata["next_dt"].dtype) if plan.rk45 is not None else None
     return plan
 
@@ -480,7 +490,7 @@ def execute_decomposed(dfs: DecomposedFieldSet, pdata: dict, kernels, dt: float,
     routed to the owners first).  Returns (local particle dict after the call, stats)."""
     plan = decomposed_plan(dfs, kernels, pdata)
     upload_decomposed(dfs, pdata, dt, plan)
-    if _carries_resume(plan):
+    if _carries_resume(plan) or dfs.fs.interp_method != "linear":
         plan.batch_levels = _global_batch_levels(dfs, pdata, dt, endtime, dist, _engine_memory_device(dfs.device))
     if dfs.fs.time_window is not None:
         # first window: where the earliest (latest, backward in time) particle of ANY rank starts -- the same on every rank

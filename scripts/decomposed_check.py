@@ -7,12 +7,13 @@ import os
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
+sys.path[:0] = [ROOT, os.path.join(ROOT, "tests"), os.path.join(ROOT, "scripts")]
 import numpy as np
 import torch
 import torch.distributed as dist
 
 import bench
+import decomposed_kernels
 import parcels_b200 as pb
 from parcels_b200 import distributed as D
 from parcels_b200.particle import create_particle_data
@@ -30,8 +31,14 @@ ap.add_argument("--time-window", type=int, default=0, help="time-slab streaming 
 ap.add_argument("--nt", type=int, default=3, help="time levels of the synthetic field (one day apart)")
 ap.add_argument("--runtime", type=float, default=86400.0)
 ap.add_argument("--diffusion", action="store_true", help="fused DiffusionUniformKh on a field at rest: statistical check (Var = 2 K t)")
-ap.add_argument("--kernel", default="rk4_3d", choices=["rk4_3d", "rk45", "m1", "em"],
-                help="rk45 / m1 / em: [AdvectionRK45 | AdvectionDiffusionM1 | EM, DeleteParticle] (scripts/decomposed_kernels.py)")
+ap.add_argument("--kernel", default="rk4_3d", choices=list(decomposed_kernels.KERNELS),
+                help="[AdvectionRK4 | RK4_3D | RK45 | AdvectionDiffusionM1 | EM, DeleteParticle]; anything but the default XLinear_Velocity "
+                "RK4_3D run on a spherical mesh takes its case from scripts/decomposed_kernels.py")
+ap.add_argument("--interp", default="linear", choices=list(decomposed_kernels.INTERP),
+                help="vector interpolator of the slabs: XLinear_Velocity, CGrid_Velocity, XFreeslip, XPartialslip, nearest node")
+ap.add_argument("--dt", type=float, default=600.0, help="time step in seconds (RK45: the initial one)")
+ap.add_argument("--f32-coords", action="store_true", help="float32 lon / lat / depth")
+ap.add_argument("--ordered-releases", action="store_true", help="delayed releases in the order of the particle ids")
 ap.add_argument("--mesh", default="spherical", choices=["spherical", "flat"])
 ap.add_argument("--backward", action="store_true")
 ap.add_argument("--delayed", action="store_true", help="releases at three different times")
@@ -61,7 +68,8 @@ if a.diffusion:
     x, y, z = np.zeros(n), np.zeros(n), np.full(n, 100.0)
     full = create_particle_data(nparticles=n, ngrids=2, initial=dict(x=x, y=y, z=z, t=np.zeros(n), particle_id=np.arange(n)))
     dfs = D.DecomposedFieldSet(lon=f["lon"], lat=f["lat"], depth=f["depth"], time=f["times"], U=f["U"], V=f["V"], W=f["W"],
-                               mesh="spherical", rank=rank, world=world, halo_cells=a.halo, device=dev)
+                               mesh="spherical", rank=rank, world=world, halo_cells=a.halo, device=dev,
+                               **decomposed_kernels.fieldset_kwargs(a.interp))  # fmt: skip
     dfs.fs.add_constant_field("Kh_zonal", K, mesh="spherical")
     dfs.fs.add_constant_field("Kh_meridional", K, mesh="spherical")
     if p2p:
@@ -81,12 +89,11 @@ if a.diffusion:
     dist.barrier()
     dist.destroy_process_group()
     sys.exit(0 if ok else 1)
-if a.kernel != "rk4_3d":
-    sys.path.insert(0, os.path.join(ROOT, "scripts"))
-    import decomposed_kernels
-
+if (a.kernel != "rk4_3d" or a.interp != "linear" or a.mesh != "spherical" or a.backward or a.delayed or a.f32_coords
+        or a.ordered_releases or a.dt != 600.0):  # fmt: skip
     case = decomposed_kernels.make_case(a.kernel, mesh=a.mesh, n=n, nt=a.nt, runtime=a.runtime, backward=a.backward,
-                                        delayed=a.delayed or bool(a.time_window), max_dt=a.max_dt, dres=a.dres, tol=a.rk45_tol)  # fmt: skip
+                                        delayed=a.delayed or bool(a.time_window), max_dt=a.max_dt, dres=a.dres, tol=a.rk45_tol,
+                                        interp=a.interp, f32_coords=a.f32_coords, dt=a.dt, ordered=a.ordered_releases)  # fmt: skip
     dfs = decomposed_kernels.decomposed_fieldset(case, rank, world, halo=a.halo, time_window=a.time_window or None, device=dev)
     if p2p:
         D.connect_p2p(dfs, dist, a.inbox or n)
@@ -104,7 +111,7 @@ if a.kernel != "rk4_3d":
         ref = decomposed_kernels.reference(case, device=dev)
         ok, msgs = decomposed_kernels.compare(merged, ref, a.kernel)
         print("\n".join(msgs))
-        print(f"decomposed {a.kernel} ({world} ranks, backend={dist.get_backend()}, {a.mesh}{', backward' if a.backward else ''}): "
+        print(f"decomposed {a.kernel} ({a.interp}, {world} ranks, backend={dist.get_backend()}, {a.mesh}{', backward' if a.backward else ''}): "
               f"{len(ref['x'])} of {n} left, {int(tot)} migrations, rounds={stats['rounds']}, transport={stats['transport']}"
               + (f", time window {a.time_window} of {a.nt} levels" if a.time_window else "") + f" -> {'PASS bit-exact' if ok else 'FAIL'}")  # fmt: skip
     dist.barrier()

@@ -1,7 +1,8 @@
-"""Cases of AdvectionRK45 and AdvectionDiffusionM1 / EM under mode D, shared by scripts/decomposed_check.py (gloo / NCCL ranks) and
-scripts/decomposed_threads_check.py (thread ranks, in-kernel migration): the config-2 field shape at 3-degree resolution, fast
-enough that particles cross slab edges several times a day, and the undecomposed single-engine run the decomposed one must equal
-bit for bit (ids, x, y, z, t, state, ei; RK45 also dt and next_dt)."""
+"""Cases of mode D beyond the default XLinear_Velocity RK4_3D run, shared by scripts/decomposed_check.py (gloo / NCCL ranks) and
+scripts/decomposed_threads_check.py (thread ranks, in-kernel migration): the fixed-step RK4 / RK4_3D, AdvectionRK45 and
+AdvectionDiffusionM1 / EM on the config-2 field shape at 3-degree resolution, fast enough that particles cross slab edges several
+times a day, with any of the vector interpolators a slab can run (``INTERP``), and the undecomposed single-engine run the
+decomposed one must equal bit for bit (ids, x, y, z, t, state, ei; RK45 also dt and next_dt)."""
 import os
 import sys
 
@@ -14,22 +15,49 @@ import bench
 import parcels_b200 as pb
 from parcels_b200.particle import create_particle_data
 
-KERNELS = {"rk45": pb.AdvectionRK45, "m1": pb.AdvectionDiffusionM1, "em": pb.AdvectionDiffusionEM}
+KERNELS = {"rk4": pb.AdvectionRK4, "rk4_3d": pb.AdvectionRK4_3D, "rk45": pb.AdvectionRK45, "m1": pb.AdvectionDiffusionM1,
+           "em": pb.AdvectionDiffusionEM}  # fmt: skip
+# --interp of the scripts -> FieldSet.from_arrays' interp_method; C-grids take the SGRID padding of NEMO-like output
+INTERP = {"linear": "linear", "cgrid": "cgrid_velocity", "freeslip": "freeslip", "partialslip": "partialslip", "nearest": "nearest"}
+# land (U = V = W = 0) for the slip and nearest-node cases: blocks of columns around the interior slab edges of 2 and 3 slabs
+# (nodes 60; 40 and 79 of 120), so that the slip factors act where particles cross from one slab to the next
+LAND_COLUMNS = [slice(36, 45), slice(56, 65), slice(75, 84)]
+LAND_ROWS = slice(20, 41)
+
+
+def fieldset_kwargs(interp):
+    kw = dict(interp_method=INTERP[interp])
+    if interp == "cgrid":
+        kw["padding"] = ("low", "low", "high")
+    return kw
+
+
 NEXT_DT = pb.Particle.add_variable(pb.Variable("next_dt", dtype=np.float32, initial=0))
 
 
 def make_case(kernel, *, mesh="spherical", n=1000, nt=3, runtime=86400.0, backward=False, delayed=False, max_dt=3600.0, dres=0.05,
-              tol=100.0, seed=7):  # fmt: skip
+              tol=100.0, seed=7, interp="linear", f32_coords=False, dt=600.0, ordered=False):  # fmt: skip
+    """``ordered``: delayed releases in the order of the particle ids, so that the first shards hold only particles on the first
+    time level and the batch-level bits of the call's first evaluation must come from the whole set."""
     f = bench.c2_field(nx=120, ny=60, nz=12, nt=nt)
-    # ~40 m/s on the sphere (~30 degrees a day); the same displacement in mesh units on a flat mesh
-    scale = np.float32(40.0 if mesh == "spherical" else 40.0 / 111319.49)
+    # ~40 m/s on the sphere (~30 degrees a day); the same displacement in mesh units on a flat mesh -- and with nearest-node
+    # sampling, which converts no units: its values are degrees per second on the sphere too
+    scale = np.float32(40.0 if mesh == "spherical" and interp != "nearest" else 40.0 / 111319.49)
     f["U"] *= scale
     f["V"] *= scale
+    if interp in ("freeslip", "partialslip", "nearest"):
+        for k in "UVW":
+            for cols in LAND_COLUMNS:
+                f[k][:, :, LAND_ROWS, cols] = 0
+    if f32_coords:
+        for k in ("lon", "lat", "depth"):
+            f[k] = f[k].astype(np.float32)
     rng = np.random.default_rng(seed)
     x, y, z = rng.uniform(-175, 175, n), rng.uniform(-70, 70, n), rng.uniform(5, 5000, n)
-    dt = -600.0 if backward else 600.0
+    dt = -abs(dt) if backward else abs(dt)
     t_start = float(f["times"][-1]) if backward else 0.0
-    t = t_start + np.sign(dt) * (rng.choice([0.0, 7200.0, 40000.0], n) if delayed else np.zeros(n))
+    delays = rng.choice([0.0, 7200.0, 40000.0], n) if delayed or ordered else np.zeros(n)
+    t = t_start + np.sign(dt) * (np.sort(delays) if ordered else delays)
     endtime = t_start + np.sign(dt) * runtime
     context = {"dres": float(dres)}
     if kernel == "rk45":
@@ -48,7 +76,7 @@ def make_case(kernel, *, mesh="spherical", n=1000, nt=3, runtime=86400.0, backwa
         full["next_dt"] = np.zeros(n, dtype=np.float32)
     kernels = [KERNELS[kernel], pb.DeleteParticle]
     return dict(kernel=kernel, f=f, mesh=mesh, x=x, y=y, z=z, t=t, dt=dt, endtime=endtime, full=full, kernels=kernels,
-                context=context, kh=(kh, np.ascontiguousarray(kh[..., ::-1])), seed=11)  # fmt: skip
+                context=context, kh=(kh, np.ascontiguousarray(kh[..., ::-1])), seed=11, fs_kw=fieldset_kwargs(interp))  # fmt: skip
 
 
 def setup(fs, case, time_window=None):
@@ -65,7 +93,8 @@ def decomposed_fieldset(case, rank, world, halo=1, time_window=None, device=0):
 
     f = case["f"]
     dfs = D.DecomposedFieldSet(lon=f["lon"], lat=f["lat"], depth=f["depth"], time=f["times"], U=f["U"], V=f["V"], W=f["W"],
-                               mesh=case["mesh"], rank=rank, world=world, halo_cells=halo, device=device, time_window=time_window)  # fmt: skip
+                               mesh=case["mesh"], rank=rank, world=world, halo_cells=halo, device=device, time_window=time_window,
+                               **case["fs_kw"])  # fmt: skip
     setup(dfs, case, time_window)
     return dfs
 
@@ -74,7 +103,7 @@ def reference(case, device=0) -> dict:
     """The single-engine run with every time level resident."""
     f = case["f"]
     fs = pb.FieldSet.from_arrays(lon=f["lon"], lat=f["lat"], depth=f["depth"], time=f["times"], U=f["U"], V=f["V"], W=f["W"],
-                                 mesh=case["mesh"])  # fmt: skip
+                                 mesh=case["mesh"], **case["fs_kw"])  # fmt: skip
     setup(fs, case)
     pclass = NEXT_DT if case["kernel"] == "rk45" else pb.Particle
     ps = pb.ParticleSet(fs, pclass=pclass, x=case["x"], y=case["y"], z=case["z"], t=case["t"], device=device, seed=case["seed"])

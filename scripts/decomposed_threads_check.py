@@ -31,22 +31,28 @@ def main():
     ap.add_argument("--nt", type=int, default=3)
     ap.add_argument("--runtime", type=float, default=86400.0)
     ap.add_argument("--backward", action="store_true")
-    ap.add_argument("--kernel", default="rk4_3d", choices=["rk4_3d", *decomposed_kernels.KERNELS],
-                    help="rk45 / m1 / em: [AdvectionRK45 | AdvectionDiffusionM1 | EM, DeleteParticle] (scripts/decomposed_kernels.py)")
+    ap.add_argument("--kernel", default="rk4_3d", choices=list(decomposed_kernels.KERNELS),
+                    help="[AdvectionRK4 | RK4_3D | RK45 | AdvectionDiffusionM1 | EM, DeleteParticle]; anything but the default "
+                    "XLinear_Velocity RK4_3D run on a spherical mesh takes its case from scripts/decomposed_kernels.py")
+    ap.add_argument("--interp", default="linear", choices=list(decomposed_kernels.INTERP),
+                    help="vector interpolator of the slabs: XLinear_Velocity, CGrid_Velocity, XFreeslip, XPartialslip, nearest node")
+    ap.add_argument("--dt", type=float, default=600.0, help="time step in seconds (RK45: the initial one)")
+    ap.add_argument("--f32-coords", action="store_true", help="float32 lon / lat / depth")
+    ap.add_argument("--ordered-releases", action="store_true", help="delayed releases in the order of the particle ids")
     ap.add_argument("--mesh", default="spherical", choices=["spherical", "flat"])
     ap.add_argument("--delayed", action="store_true", help="releases at three different times")
     ap.add_argument("--halo", type=int, default=3)
     ap.add_argument("--max-dt", type=float, default=3600.0, help="RK45_max_dt")
     a = ap.parse_args()
     world, n = a.world, a.particles
-    if a.kernel != "rk4_3d":
+    if a.kernel != "rk4_3d" or a.interp != "linear" or a.mesh != "spherical" or a.delayed or a.f32_coords or a.ordered_releases:
         return kernel_case(a)
     f = bench.c2_field(nx=120, ny=60, nz=12, nt=a.nt)
     f["U"] *= np.float32(40.0)
     f["V"] *= np.float32(40.0)
     rng = np.random.default_rng(7)
     x, y, z = rng.uniform(-175, 175, n), rng.uniform(-70, 70, n), rng.uniform(5, 5000, n)
-    dt = -600.0 if a.backward else 600.0
+    dt = -a.dt if a.backward else a.dt
     t_start = float(f["times"][-1]) if a.backward else 0.0
     # staggered releases: particles wait at different times, the lock-step slide has to serve the earliest first
     t = t_start + np.sign(dt) * rng.choice([0.0, 7200.0, 100800.0], n) if a.time_window else np.full(n, t_start)
@@ -54,7 +60,8 @@ def main():
     kernels = [pb.AdvectionRK4_3D, pb.DeleteParticle]
     full = create_particle_data(nparticles=n, ngrids=1, initial=dict(x=x, y=y, z=z, t=t, particle_id=np.arange(n)))
     slabs = [D.DecomposedFieldSet(lon=f["lon"], lat=f["lat"], depth=f["depth"], time=f["times"], U=f["U"], V=f["V"], W=f["W"],
-                                  mesh="spherical", rank=r, world=world, halo_cells=3, device=0, time_window=a.time_window or None)
+                                  mesh="spherical", rank=r, world=world, halo_cells=a.halo, device=0,
+                                  time_window=a.time_window or None)
              for r in range(world)]  # fmt: skip
     bases = [s.engine.migrate_p2p_init(a.inbox or n)[1] for s in slabs]
     for s in slabs:
@@ -86,7 +93,8 @@ def main():
 
 def kernel_case(a):
     case = decomposed_kernels.make_case(a.kernel, mesh=a.mesh, n=a.particles, nt=a.nt, runtime=a.runtime, backward=a.backward,
-                                        delayed=a.delayed or bool(a.time_window), max_dt=a.max_dt)  # fmt: skip
+                                        delayed=a.delayed or bool(a.time_window), max_dt=a.max_dt, interp=a.interp,
+                                        f32_coords=a.f32_coords, dt=a.dt, ordered=a.ordered_releases)  # fmt: skip
     world, n = a.world, a.particles
     slabs = [decomposed_kernels.decomposed_fieldset(case, r, world, halo=a.halo, time_window=a.time_window or None) for r in range(world)]
     bases = [s.engine.migrate_p2p_init(a.inbox or n)[1] for s in slabs]
@@ -103,7 +111,7 @@ def kernel_case(a):
     ok, msgs = decomposed_kernels.compare(merged, ref, a.kernel)
     print("\n".join(msgs))
     migrated = sum(s["migrated"] for s in stats)
-    print(f"decomposed {a.kernel} ({world} thread ranks, {a.mesh}{', backward' if a.backward else ''}): {len(ref['x'])} of {n} left, "
+    print(f"decomposed {a.kernel} ({a.interp}, {world} thread ranks, {a.mesh}{', backward' if a.backward else ''}): {len(ref['x'])} of {n} left, "
           f"{migrated} migrations, rounds={stats[0]['rounds']}, transport={stats[0]['transport']}"
           + (f", time window {a.time_window} of {a.nt} levels" if a.time_window else "") + f" -> {'PASS bit-exact' if ok else 'FAIL'}")  # fmt: skip
     return 0 if ok else 1
