@@ -1365,6 +1365,18 @@ int32_t pb_advect(pb_engine* e, const pb_advect_args* a, pb_report* rep) {
     return PB_OK;
 }
 
+// rk45_kernel for the engine's velocity interpolator: CGrid_Velocity, XFreeslip / XPartialslip or XLinear_Velocity
+static cudaError_t launch_rk45_kernel(const pb_engine* e, const AdvectParams& p, const pb_rk45_args* a, double* dt, double* next_dt,
+                                      int* iters) {
+    const bool coord_f64 = e->coord_f64 != 0, data_f64 = e->f_f64[0] != 0;
+    if (e->interp == PB_INTERP_CGRID_VELOCITY)
+        return launch_rk45_cgrid(p, dt, next_dt, iters, a->next_dt_is_f32, a->tol, a->min_dt, a->max_dt, coord_f64, data_f64, e->stream);
+    if (agrid_alt_mode(e->interp) == 1)
+        return launch_rk45_slip(p, dt, next_dt, iters, a->next_dt_is_f32, a->tol, a->min_dt, a->max_dt, coord_f64, data_f64, e->g.nt > 0,
+                                e->stream);
+    return launch_rk45(p, dt, next_dt, iters, a->next_dt_is_f32, a->tol, a->min_dt, a->max_dt, coord_f64, data_f64, e->g.nt > 0, e->stream);
+}
+
 int32_t pb_advect_rk45(pb_engine* e, const pb_rk45_args* a, double* dt_inout, double* next_dt_inout, pb_report* rep) {
     PB_RANGE("pb_advect_rk45");
     if (!e || !a || !rep) return fail(PB_ERR_INVALID, "NULL argument");
@@ -1395,12 +1407,7 @@ int32_t pb_advect_rk45(pb_engine* e, const pb_rk45_args* a, double* dt_inout, do
     p.lone_particle = e->n == 1;
     if ((rc = begin_launch(e))) return rc;
     if (n) {
-        cudaError_t ce = cgrid ? launch_rk45_cgrid(p, d_dt, d_ndt, d_it, a->next_dt_is_f32, a->tol, a->min_dt, a->max_dt, e->coord_f64 != 0,
-                                                   e->f_f64[0] != 0, e->stream)
-                         : slip ? launch_rk45_slip(p, d_dt, d_ndt, d_it, a->next_dt_is_f32, a->tol, a->min_dt, a->max_dt, e->coord_f64 != 0,
-                                                  e->f_f64[0] != 0, e->g.nt > 0, e->stream)
-                                : launch_rk45(p, d_dt, d_ndt, d_it, a->next_dt_is_f32, a->tol, a->min_dt, a->max_dt, e->coord_f64 != 0,
-                                              e->f_f64[0] != 0, e->g.nt > 0, e->stream);
+        cudaError_t ce = launch_rk45_kernel(e, p, a, d_dt, d_ndt, d_it);
         if (ce != cudaSuccess) return fail(PB_ERR_CUDA, "rk45_kernel launch failed: %s", cudaGetErrorString(ce));
     }
     if ((rc = end_launch(e))) return rc;
@@ -1443,12 +1450,7 @@ int32_t pb_advect_rk45_resident_async(pb_engine* e, const pb_rk45_args* a) {
     if ((rc = begin_launch(e))) return rc;
     if (e->n > 0) {
         const ResumeDev r = e->cur.resume();
-        cudaError_t ce = cgrid ? launch_rk45_cgrid(p, r.dt, r.next_dt, r.iters, a->next_dt_is_f32, a->tol, a->min_dt, a->max_dt,
-                                                   e->coord_f64 != 0, e->f_f64[0] != 0, e->stream)
-                         : slip ? launch_rk45_slip(p, r.dt, r.next_dt, r.iters, a->next_dt_is_f32, a->tol, a->min_dt, a->max_dt,
-                                                  e->coord_f64 != 0, e->f_f64[0] != 0, e->g.nt > 0, e->stream)
-                                : launch_rk45(p, r.dt, r.next_dt, r.iters, a->next_dt_is_f32, a->tol, a->min_dt, a->max_dt,
-                                              e->coord_f64 != 0, e->f_f64[0] != 0, e->g.nt > 0, e->stream);
+        cudaError_t ce = launch_rk45_kernel(e, p, a, r.dt, r.next_dt, r.iters);
         if (ce != cudaSuccess) return fail(PB_ERR_CUDA, "rk45_kernel launch failed: %s", cudaGetErrorString(ce));
     }
     return end_launch(e);

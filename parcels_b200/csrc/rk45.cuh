@@ -20,10 +20,7 @@ template <class Policy>
 __global__ void __launch_bounds__(PB_BLOCK_THREADS, PB_MINBLOCKS) rk45_kernel(const Rk45Params q) {
     const AdvectParams& p = q.base;
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    unsigned long long my_steps = 0, my_evals = 0;
-    long long my_iters = 0;
-    bool stalled = false, wait_window = false, migrate = false, halo = false;
-    int final_state = 0;
+    LaneTally tally;  // refills: the number of field evaluations (6 per attempt)
     if (i < p.P.n) {
         // Butcher tableau of _advection.py:96-106, the same Python float expressions
         const double c[5] = {1.0 / 4.0, 3.0 / 8.0, 12.0 / 13.0, 1.0, 1.0 / 2.0};
@@ -35,20 +32,20 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, PB_MINBLOCKS) rk45_kernel(co
         const double b4[5] = {25.0 / 216.0, 0.0, 1408.0 / 2565.0, 2197.0 / 4104.0, -1.0 / 5.0};
         const double b5[6] = {16.0 / 135.0, 0.0, 6656.0 / 12825.0, 28561.0 / 56430.0, -9.0 / 50.0, 2.0 / 55.0};
 
-        float x = p.P.x[i], y = p.P.y[i], z = p.P.z[i];
-        float dx = p.P.dx[i], dy = p.P.dy[i], dz = p.P.dz[i];
-        double t = p.P.t[i];
+        Lane L = load_lane(p, i);
+        float &x = L.x, &y = L.y, &z = L.z, &dx = L.dx, &dy = L.dy, &dz = L.dz;
+        double& t = L.t;
         double dt = q.dt[i], ndt = q.next_dt[i];
         typename Policy::Ctx e;
         Policy::init(e, p, p.P.ei[i]);
-        e.state = p.resume ? p.P.state[i] : (int)PB_EVALUATE;  // kernel.py:188
+        e.state = initial_state(p, i);
         e.refills = 0;
         e.out_of_time = false;
         if constexpr (Policy::BATCH_LEN_Z) {
             if (p.batch_levels & PB_BATCH_TWO_Z) e.len_z = 1;
         }
         const int sign = p.dt > 0 ? 1 : -1;  // compute_time_direction (kernel.py:186)
-        bool first_attempt = true;
+        bool first_attempt = true, halo = false;
         // a resumed launch of the same Kernel.execute call (time-slab streaming) continues the lane's iteration count, so the
         // first-iteration batch rules, max_iters and the finalize clamp see the iterations of the whole call
         long long it = (p.resume && !p.kernels_only) ? (long long)q.iters[i] : 0;
@@ -56,29 +53,24 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, PB_MINBLOCKS) rk45_kernel(co
             if (p.max_iters >= 0 && it >= p.max_iters) break;
             const double tte = sign * (p.endtime - t);
             if (!((e.state == PB_SUCCESS || e.state == PB_EVALUATE) && tte >= 0)) break;
-            // mode D: not ours (any more).  Tested before the window wait, as in advect_kernel: the new owner, whose window slides in
-            // lock-step with this one, makes the same wait decision
+            // mode D: not ours (any more).  Tested before the window wait: the new owner, whose window slides in lock-step with this
+            // one, makes the same wait decision
             if (p.g.decomposed && !((double)x >= p.g.own_lo && (double)x < p.g.own_hi)) {
-                migrate = true;
+                tally.migrate = true;
                 break;
             }
-            dt = (sign == 1) ? fmax(fmin(dt, tte), 0.0) : fmin(fmax(dt, -tte), 0.0);  // kernel.py:199-203
+            dt = clamp_dt(dt, tte, sign);
             if (dt == 0.0 && tte > 0) {  // the reference never terminates here (t cannot advance): report instead of spinning
-                stalled = true;
+                tally.stalled = true;
                 break;
             }
-            if (p.f.windowed) {
-                // every attempt of this iteration samples inside [t, t + dt] (a rejected attempt halves dt), so that span must
-                // lie within the resident time levels; outside the field's whole time interval is OutsideTimeInterval, not a wait
-                const double ta = fmin(t, t + dt), tb = fmax(t, t + dt);
-                if (!(ta >= p.f.win_t0 && tb <= p.f.win_t1) && ta >= 0 && tb <= p.g.time_len) {
-                    wait_window = true;  // state, dt and next_dt stay as they are: the resumed launch repeats this iteration
-                    atomicMin(&p.rep->wait_t_min_bits, (unsigned long long)__double_as_longlong(t));
-                    atomicMax(&p.rep->wait_t_max_bits, (unsigned long long)__double_as_longlong(t));
-                    break;
-                }
+            // every attempt of this iteration samples inside [t, t + dt] (a rejected attempt halves dt); a wait leaves state, dt and
+            // next_dt as they are
+            if (window_wait(p, t, t + dt, t)) {
+                tally.wait_window = true;
+                break;
             }
-            my_steps++;
+            tally.steps++;
             do {  // kernel.py:206-216: the kernel, then again for as long as it asks to be repeated
                 const double sgn_dt = dt > 0 ? 1.0 : (dt < 0 ? -1.0 : 0.0);  // np.sign(particles.dt)
                 Val u[6], v[6], wdummy;
@@ -121,7 +113,7 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, PB_MINBLOCKS) rk45_kernel(co
                     Policy::template eval<float, double, double>(p, e, false, t + c[k] * dt, z, ys, xs, u[k + 1], v[k + 1], wdummy);
                 }
                 }
-                my_evals += 6;
+                tally.refills += 6;
                 // mode D: a stage position left the owned + halo columns (state 99, which the line `e.state = good ? ...` below
                 // would overwrite): the lane stops with it
                 if (p.g.decomposed && e.state == 99) {
@@ -168,46 +160,16 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, PB_MINBLOCKS) rk45_kernel(co
             if (e.state == PB_EVALUATE && t == p.endtime) e.state = PB_END_OF_LOOP;
         }
         Policy::finish(e, p);
-        my_iters = it;
-        final_state = stalled ? (int)PB_ERROR : e.state;
-        p.P.x[i] = x; p.P.y[i] = y; p.P.z[i] = z;
-        p.P.dx[i] = dx; p.P.dy[i] = dy; p.P.dz[i] = dz;
-        p.P.t[i] = t;
-        p.P.state[i] = final_state;
-        p.P.ei[i] = e.ei;
+        tally.iters = it;
+        tally.state = tally.stalled ? (int)PB_ERROR : e.state;
+        store_lane(p, i, L, tally.state, e.ei);
         q.dt[i] = dt;
         q.next_dt[i] = ndt;
         q.iters[i] = (int)it;
-        if (migrate && p.mig.on) {
-            MigRecord rec;
-            rec.t = t; rec.pid = p.P.pid[i];
-            rec.x = x; rec.y = y; rec.z = z; rec.dx = dx; rec.dy = dy; rec.dz = dz;
-            rec.state = final_state; rec.ei = e.ei;
-            migrate = mig_deliver(p, i, rec, MigResume{dt, ndt, (int)it, 0});
+        if (tally.migrate && p.mig.on) {
+            const MigResume rs{dt, ndt, (int)it, 0};
+            tally.migrate = mig_deliver(p, i, L, tally.state, e.ei, &rs);
         }
     }
-    const unsigned full = 0xffffffffu;
-    unsigned long long s_steps = my_steps, s_ev = my_evals;
-    unsigned n_stall = stalled, n_ww = wait_window, n_mig = migrate;
-    long long mx_it = my_iters;
-    int mx_state = final_state;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        s_steps += __shfl_xor_sync(full, s_steps, o);
-        s_ev += __shfl_xor_sync(full, s_ev, o);
-        n_stall += __shfl_xor_sync(full, n_stall, o);
-        n_ww += __shfl_xor_sync(full, n_ww, o);
-        n_mig += __shfl_xor_sync(full, n_mig, o);
-        mx_it = max(mx_it, __shfl_xor_sync(full, mx_it, o));
-        mx_state = max(mx_state, __shfl_xor_sync(full, mx_state, o));
-    }
-    if ((threadIdx.x & 31) == 0) {
-        if (s_steps) atomicAdd(&p.rep->particle_steps, s_steps);
-        if (s_ev) atomicAdd(&p.rep->cache_refills, s_ev);  // RK45: the number of field evaluations (6 per attempt)
-        if (n_stall) atomicAdd(&p.rep->n_error, (unsigned long long)n_stall);
-        if (n_ww) atomicAdd(&p.rep->n_wait_window, (unsigned long long)n_ww);
-        if (n_mig) atomicAdd(&p.rep->n_migrate, (unsigned long long)n_mig);
-        if (mx_it) atomicMax(&p.rep->max_iters_done, mx_it);
-        if (mx_state) atomicMax(&p.rep->max_state, mx_state);
-    }
+    publish(tally, p.rep);
 }

@@ -14,7 +14,7 @@ lenZ pre-pass all pass it.  This file checks those on the device:
    released later) in a set that never does -- and one hit-path particle among missing lanes -- at lanes 0, 1 and 31 of a
    warp, in the first and last warp of a block and in the first and last block: bit-identical wherever it sits, its
    neighbours unchanged, and equal to the oracle (bit for bit in engine arithmetic);
-3. warp-reduced reports against a recount from the returned arrays;
+3. warp-reduced reports against a recount from the returned arrays (the headline RK4 kernel and AdvectionDiffusionM1);
 4. the batch flags (`any(tau > 0)`, `any(zeta > 0)`) of pb_sample_velocity / pb_sample_scalar when the one sample that sets
    them sits at a lane / warp / block boundary of the pre-pass.
 
@@ -454,9 +454,20 @@ def _oracle_with_ids(c, ids):
 # ------------------------------------------------------------------------------------------------
 # 3. warp-reduced reports against a per-particle recount
 # ------------------------------------------------------------------------------------------------
-def _report_case(n, delete, rng):
-    spec = dict(cases.CASES["c2_small"], mesh="flat", umax=8.0, n=8, segments=[dict(endtime=2400.0)], delete=delete)
+# kernel family -> (case, environment, end time): the headline RK4 kernel and AdvectionDiffusionM1 both warp-reduce their
+# reports and take fixed steps, so the same recount holds
+REPORT_KERNELS = {"afast": ("c2_small", {"PB_DISABLE_FAST_KERNEL": "0", "PB_FAST_KERNEL": "2"}, 2400.0),
+                  "advdiff": ("flat_f32c_f64d", {}, 100.0)}  # fmt: skip
+
+
+def _report_case(n, delete, rng, kind):
+    base, _, endtime = REPORT_KERNELS[kind]
+    spec = dict(cases.CASES[base], mesh="flat", umax=8.0, n=8, segments=[dict(endtime=endtime)], delete=delete)
+    if kind == "advdiff":
+        spec.update(kernels=["AdvectionDiffusionM1"], umax=6.0)
     c = cases.build(spec)
+    if kind == "advdiff":
+        c["W"] = None
     lon, lat = np.asarray(c["lon"]), np.asarray(c["lat"])
     lx, ly = lon[-1] - lon[0], lat[-1] - lat[0]
     d = np.asarray(c["depth"], dtype=np.float64)
@@ -468,7 +479,7 @@ def _report_case(n, delete, rng):
     z = rng.uniform(d[0] + 0.3 * (d[-1] - d[0]), d[-1] - 0.3 * (d[-1] - d[0]), n)
     # every lane its own iteration count: releases at 0 .. 5 steps, and some after the end of the run (no step at all)
     t = c["dt"] * rng.integers(0, 6, n).astype(np.float64)
-    t[rng.random(n) < 0.05] = 3000.0
+    t[rng.random(n) < 0.05] = 1.25 * endtime
     t[0] = 0.0
     c.update(x=x, y=y, z=z, t=t)
     return c
@@ -487,33 +498,37 @@ def test_warp_reduced_reports_equal_a_recount_from_the_arrays(n, blocks):
     block = blocks["agrid_fast"]
     n = {"block-1": block - 1, "block+1": block + 1, "3block-1": 3 * block - 1, "3block+1": 3 * block + 1,
          "big": 9_999 if HOSTSIM else 1_000_001}.get(n, n)  # fmt: skip
+    for kind in REPORT_KERNELS:
+        _check_reports(n, kind)
+
+
+def _check_reports(n, kind):
+    _, env, endtime = REPORT_KERNELS[kind]
     rng = np.random.default_rng(n)
-    env = {"PB_DISABLE_FAST_KERNEL": "0", "PB_FAST_KERNEL": "2"}
     # (a) no errors: the steps of every lane
-    c = _report_case(n, False, rng)
-    c["segments"] = [dict(endtime=2400.0)]
-    got, err, rep = _run(c, "afast", env, np.arange(n))
+    c = _report_case(n, False, rng, kind)
+    got, err, rep = _run(c, kind, env, np.arange(n))
     assert err == "" and len(got["particle_id"]) == n
     t_in = c["t"][got["particle_id"]]
-    steps = _recount_steps(t_in, got["t"], c["dt"], 2400.0)
-    assert np.all(got["t"][t_in <= 2400.0] == 2400.0)
+    steps = _recount_steps(t_in, got["t"], c["dt"], endtime)
+    assert np.all(got["t"][t_in <= endtime] == endtime)
     assert rep[0]["particle_steps"] == int(steps.sum()), (rep[0]["particle_steps"], int(steps.sum()))
     assert rep[0]["max_iters_done"] == int(steps.max())
     assert rep[0]["n_deleted"] == 0 and rep[0]["n_error"] == 0 and rep[0]["first_error_iter"] < 0 or rep[0]["n_error"] == 0
     assert rep[0]["max_state"] == int(got["state"].max())
     # (b) with the delete handler: what was deleted is what is missing
-    c = _report_case(n, True, rng)
+    c = _report_case(n, True, rng, kind)
     c["U"] = c["U"] * np.float32(4.0)
-    got, err, rep = _run(c, "afast", env, np.arange(n))
+    got, err, rep = _run(c, kind, env, np.arange(n))
     assert err == ""
     gone = n - len(got["particle_id"])
     assert rep[0]["n_deleted"] == gone and rep[0]["n_error"] == 0
     assert rep[0]["max_state"] == max(int(got["state"].max(initial=0)), 30 if gone else 0)
     # (c) no handler: the run raises; the report counts the errored lanes and the first iteration any of them errored in
-    c = _report_case(n, True, rng)
+    c = _report_case(n, True, rng, kind)
     c["U"] = c["U"] * np.float32(4.0)
     c["delete_on_error"] = False
-    got, err, rep = _run(c, "afast", env, np.arange(n))
+    got, err, rep = _run(c, kind, env, np.arange(n))
     assert err or n < 100, "the run was meant to raise"
     if err:
         errored = got["state"] >= 50
