@@ -27,7 +27,11 @@ columns of each level (``_SlabLevels``), and the next level is copied while the 
 
 from __future__ import annotations
 
+from types import SimpleNamespace
+
 import numpy as np
+
+from .plan import KernelPlan, batch_facts, evaluated_mask
 
 
 def shard_bounds(n: int, world: int) -> list[tuple[int, int]]:
@@ -282,28 +286,24 @@ def connect_p2p(dfs: DecomposedFieldSet, dist, capacity_records: int) -> bool:
 def _carries_resume(plan) -> bool:
     """AdvectionRK45 and AdvectionDiffusionM1 / EM: a lane stopped mid-call continues on its new owner with its dt, next_dt and
     iteration count, which travel with the particle."""
-    return plan.rk45 is not None or plan.advdiff is not None
+    return plan.kind in ("rk45", "advdiff")
 
 
 def _advect_args(eng, plan, dt, endtime, first, seed, rng_call, rounds):
-    if plan.rk45 is not None:
-        return eng.make_rk45_args(dt, endtime, *plan.rk45, next_dt_is_f32=plan.next_dt_dtype == np.float32, delete_on_error=True,
-                                  resume=not first, batch_levels=plan.batch_levels)  # fmt: skip
-    if plan.advdiff is not None:
-        # the iteration count travels with the particle and keys its Wiener increments: the single-GPU run's stream, unchanged by
-        # where the rounds cut the call (no round number in the call index)
-        return eng.make_advdiff_args(dt=dt, endtime=endtime, delete_on_error=True, seed=seed, rng_call=rng_call, resume=not first,
-                                     batch_levels=plan.batch_levels, **plan.advdiff)  # fmt: skip
-    # fused DiffusionUniformKh: the Wiener increments are keyed by (seed; particle id, iteration of the launch, call index).  Every
-    # migration round is a new launch on every rank (the round count is global), so the round number joins the call index and no
-    # particle ever draws the same increment twice, wherever it migrates.  (The stream differs from a single-GPU run's, whose
-    # iterations are not cut into rounds: statistically equivalent, not bit-identical -- the advection-only path is.)
-    # The fixed-step kernel restarts its iteration count in every launch, so the first-evaluation time bit reaches the first
-    # iteration of every round.  That is the single-GPU rule: the bit changes a value only on the first time level (tau == 0), where
-    # a particle is before its first step -- a lane the first round only routed to its owner, or one that waited for the window.
-    return eng.make_args(plan.scheme, dt, endtime, delete_on_error=True, resume=not first, diffusion=plan.diffusion, kh=plan.kh,
-                         kh_spherical=plan.kh_spherical, kh_deg2m=plan.kh_deg2m, seed=seed, rng_call=(int(rng_call) << 20) + rounds,
-                         batch_levels=plan.batch_levels)  # fmt: skip
+    """The arguments of a round's launch.  AdvectionDiffusionM1 / EM: the iteration count travels with the particle and keys its
+    Wiener increments -- the single-GPU run's stream, unchanged by where the rounds cut the call (no round number in the call index).
+
+    Fused DiffusionUniformKh: the Wiener increments are keyed by (seed; particle id, iteration of the launch, call index).  Every
+    migration round is a new launch on every rank (the round count is global), so the round number joins the call index and no
+    particle ever draws the same increment twice, wherever it migrates.  (The stream differs from a single-GPU run's, whose
+    iterations are not cut into rounds: statistically equivalent, not bit-identical -- the advection-only path is.)
+    The fixed-step kernel restarts its iteration count in every launch, so the first-evaluation time bit reaches the first
+    iteration of every round.  That is the single-GPU rule: the bit changes a value only on the first time level (tau == 0), where
+    a particle is before its first step -- a lane the first round only routed to its owner, or one that waited for the window."""
+    if plan.kind == "fixed":
+        rng_call = (int(rng_call) << 20) + rounds
+    return plan.launch_args(eng, dt, endtime, seed=seed, rng_call=rng_call, resume=not first, batch_levels=plan.batch_levels,
+                            next_dt_dtype=plan.next_dt_dtype)  # fmt: skip
 
 
 def _advect_round(dfs, args, sign):
@@ -376,7 +376,7 @@ def run_decomposed_p2p(dfs: DecomposedFieldSet, plan, dt: float, endtime: float,
 def _finish_call(dfs, plan, dt, endtime, dist, device, stats):
     """AdvectionRK45: the batch-level dt clamp of the particles that left the loop early needs the call's iteration count over
     every rank and round -- once, on every rank, after the last round."""
-    if plan.rk45 is not None:
+    if plan.kind == "rk45":
         dfs.engine.rk45_finalize(dt, endtime, int(allreduce_max(stats.get("max_iters_done", 0), dist, _collective_device(dist, device))))
 
 
@@ -423,12 +423,8 @@ def run_decomposed_resident(dfs: DecomposedFieldSet, plan, dt: float, endtime: f
 def decomposed_plan(dfs: DecomposedFieldSet, kernels, pdata: dict | None = None):
     """The kernel list lowered for mode D: one of the fused fixed-step schemes (optionally with DiffusionUniformKh),
     ``[AdvectionRK45, DeleteParticle]`` (``pdata`` must then hold ``next_dt``) or ``[AdvectionDiffusionM1 | EM, DeleteParticle]``."""
-    from types import SimpleNamespace
-
-    from .particleset import KernelPlan
-
     # (the particle variables stand in for the ParticleClass: RK45 needs next_dt)
-    pclass = SimpleNamespace(variables=[SimpleNamespace(name=k) for k in (pdata or {})])
+    pclass = SimpleNamespace(variables=[SimpleNamespace(name=k, dtype=v.dtype) for k, v in (pdata or {}).items()])
     plan = KernelPlan(kernels, dfs.fs, pclass)
     if plan.stepwise:
         raise NotImplementedError("domain-decomposed execution runs one built-in kernel -- a fixed-step advection scheme (optionally "
@@ -437,8 +433,6 @@ def decomposed_plan(dfs: DecomposedFieldSet, kernels, pdata: dict | None = None)
     if not plan.delete_on_error:
         raise NotImplementedError("domain-decomposed execution needs the DeleteParticle handler (errors cannot be replayed "
                                   "step-exactly across ranks)")  # fmt: skip
-    plan.batch_levels = 0  # the call's batch-level bits (execute_decomposed sets them, except for fixed-step XLinear_Velocity lists)
-    plan.next_dt_dtype = np.dtype(pdata["next_dt"].dtype) if plan.rk45 is not None else None
     return plan
 
 
@@ -448,7 +442,7 @@ def upload_decomposed(dfs: DecomposedFieldSet, pdata: dict, dt: float, plan=None
     from .statuscodes import StatusCode
 
     pdata["state"][:] = StatusCode.Evaluate
-    rk45 = plan is not None and plan.rk45 is not None
+    rk45 = plan is not None and plan.kind == "rk45"
     if not rk45:
         pdata["dt"][:] = dt
     dfs.engine.upload_particles(pdata, np.ascontiguousarray(pdata["ei"][:, -1]))
@@ -461,7 +455,7 @@ def download_decomposed(dfs: DecomposedFieldSet, dt: float, ngrids=1, plan=None)
     from .statuscodes import StatusCode
 
     out = dfs.engine.download_all(ngrids=ngrids)
-    if plan is not None and plan.rk45 is not None:
+    if plan is not None and plan.kind == "rk45":
         out["dt"][:], ndt, _ = dfs.engine.download_resume(len(out["x"]))
         out["next_dt"] = ndt.astype(plan.next_dt_dtype)
     else:
@@ -475,10 +469,7 @@ def _global_batch_levels(dfs, pdata, dt, endtime, dist, device) -> int:
     shard -- so that the first-iteration rule of the kernels that count their iterations across ranks is the single-GPU one."""
     import torch
 
-    from .particleset import _batch_levels
-
-    sign = 1 if dt > 0 else -1
-    bits = _batch_levels(dfs.fs, pdata, sign * (endtime - pdata["t"]) >= 0) if len(pdata["t"]) else 0
+    _, bits = batch_facts(dfs.fs, pdata, pdata["ei"][:, -1], dt, endtime)
     v = torch.tensor([float(bits & 1), float(bits & 2)], dtype=torch.float64, device=_collective_device(dist, device))
     dist.all_reduce(v, op=dist.ReduceOp.MAX)
     return int(v[0].item() > 0) | (2 if v[1].item() > 0 else 0)
@@ -490,14 +481,14 @@ def execute_decomposed(dfs: DecomposedFieldSet, pdata: dict, kernels, dt: float,
     routed to the owners first).  Returns (local particle dict after the call, stats)."""
     plan = decomposed_plan(dfs, kernels, pdata)
     upload_decomposed(dfs, pdata, dt, plan)
-    if _carries_resume(plan) or dfs.fs.interp_method != "linear":
+    if _carries_resume(plan) or dfs.fs.interp_method != "linear":  # (fixed-step XLinear_Velocity lists keep the plan's 0)
         plan.batch_levels = _global_batch_levels(dfs, pdata, dt, endtime, dist, _engine_memory_device(dfs.device))
     if dfs.fs.time_window is not None:
         # first window: where the earliest (latest, backward in time) particle of ANY rank starts -- the same on every rank
         import torch
 
         sign = 1 if dt > 0 else -1
-        todo = sign * (endtime - pdata["t"]) >= 0
+        todo = evaluated_mask(pdata, dt, endtime)
         t0 = float((sign * pdata["t"][todo]).min()) if todo.any() else np.inf
         device = _engine_memory_device(dfs.device)
         v = torch.tensor([t0], dtype=torch.float64, device=device if dist.get_backend() == "nccl" else "cpu")

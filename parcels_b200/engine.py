@@ -240,11 +240,13 @@ class Engine:
         return _report_dict(rep)
 
     @staticmethod
-    def make_rk45_args(dt, endtime, tol, min_dt, max_dt, *, next_dt_is_f32=True, delete_on_error=False, resume=False, batch_levels=0):
+    def make_rk45_args(dt, endtime, tol, min_dt, max_dt, *, next_dt_is_f32=True, delete_on_error=False, max_iters=-1, kernels_only=False,
+                       resume=False, hint_all_zero=False, batch_levels=0):  # fmt: skip
         from ._lib import Rk45Args
 
-        return Rk45Args(float(dt), float(endtime), float(tol), float(min_dt), float(max_dt), -1, int(next_dt_is_f32),
-                        int(delete_on_error), 0, int(bool(resume)), 0, int(batch_levels))  # fmt: skip
+        return Rk45Args(float(dt), float(endtime), float(tol), float(min_dt), float(max_dt), int(max_iters), int(next_dt_is_f32),
+                        int(delete_on_error), int(bool(kernels_only)), int(bool(resume)), int(bool(hint_all_zero)),
+                        int(batch_levels))  # fmt: skip
 
     def rk45_finalize(self, dt, endtime, total_iters):
         """The batch-level dt clamp of the particles that left the RK45 loop before the call's ``total_iters`` iterations
@@ -271,17 +273,11 @@ class Engine:
                            float(dres), float(deg2m_sq), int(seed), int(rng_call), int(max_iters), int(bool(kernels_only)),
                            int(bool(resume)), int(batch_levels), 0)  # fmt: skip
 
-    def advect_rk45(self, dt, endtime, tol, min_dt, max_dt, dt_arr, next_dt_arr, *, next_dt_is_f32=True, delete_on_error=False,
-                    max_iters=-1, kernels_only=False, resume=False, hint_all_zero=False, batch_levels=0) -> dict:
-        """AdvectionRK45 + Repeat / next_dt state machine; ``dt_arr`` / ``next_dt_arr`` (float64, C-contiguous) are
-        updated in place to what the reference leaves in particles.dt / particles.next_dt."""
-        from ._lib import Rk45Args
-
-        a = Rk45Args(float(dt), float(endtime), float(tol), float(min_dt), float(max_dt), int(max_iters), int(next_dt_is_f32),
-                     int(delete_on_error), int(bool(kernels_only)), int(bool(resume)), int(bool(hint_all_zero)),
-                     int(batch_levels))  # fmt: skip
+    def advect_rk45(self, args, dt_arr, next_dt_arr) -> dict:
+        """AdvectionRK45 + Repeat / next_dt state machine (``args`` from :meth:`make_rk45_args`); ``dt_arr`` / ``next_dt_arr``
+        (float64, C-contiguous) are updated in place to what the reference leaves in particles.dt / particles.next_dt."""
         rep = Report()
-        check(self._lib.pb_advect_rk45(self._h, C.byref(a), ptr(dt_arr), ptr(next_dt_arr), C.byref(rep)))
+        check(self._lib.pb_advect_rk45(self._h, C.byref(args), ptr(dt_arr), ptr(next_dt_arr), C.byref(rep)))
         return _report_dict(rep)
 
     def advect_host(self, args: AdvectArgs, d: dict, ei_last: np.ndarray, *, download: bool, n_chunks: int) -> dict:

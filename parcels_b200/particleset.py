@@ -10,12 +10,11 @@ from __future__ import annotations
 
 import datetime
 import os
-import types
 
 import numpy as np
 
-from . import kernels as K
 from .particle import _CORE, Particle, ParticleClass, create_particle_data
+from .plan import KernelPlan, _min_or_max, batch_facts, evaluated_mask
 from .statuscodes import ERRORS_TO_THROW, StatusCode, raise_for_state
 
 __all__ = ["Kernel", "ParticleSet"]
@@ -45,12 +44,6 @@ def _fill(a, value):
             _lib.check(lib.pb_host_fill_i32(_lib.ptr(a), a.size, int(value)))
     else:
         a[:] = value
-
-
-def _min_or_max(t, want_min: bool) -> float:
-    """``t.min()`` / ``t.max()`` with NumPy's NaN propagation (any NaN -> NaN), as the reference takes them (particleset.py:541-544).
-    (NumPy's own SIMD reduction: 3.5 ms for 1e7 values; a threaded scalar loop in the library measured 15 ms.)"""
-    return float(t.min() if want_min else t.max())
 
 
 def _fill_dt(pset, d, dt):
@@ -140,252 +133,33 @@ def _has_nan(a) -> bool:
     return bool(s != s) and bool(np.isnan(a).any())
 
 
-def _first_eval_two_levels(fieldset, t, evaluated) -> bool:
-    """float32 grids with a time axis: True when some evaluated particle is NOT exactly on the first time level.  The reference
-    decides `lenT = 2 if any(tau > 0)` for the whole batch of an evaluation (_xinterpolators.py:130); tau == 0 only AT the first
-    level (`_search_1d_array` is left-sided: any later level gives tau == 1), so only the first evaluation of a call can mix the
-    two cases -- and there a two-level batch promotes the value of a first-level particle to float64.  On float64 grids every
-    barycentric coordinate is float64 and the promotion changes nothing."""
-    if fieldset._time_s is None or fieldset.grid.lon.dtype != np.float32:
-        return False
-    t0 = float(fieldset._time_s[0])
-    if t.size >= (1 << 20) and _min_or_max(t, True) == t0 and _min_or_max(t, False) == t0:
-        return False  # every particle sits on the first level (the usual fresh set): no masked copies of a large column
-    te = t[evaluated() if callable(evaluated) else evaluated]
-    return bool(te.size) and bool(np.any(te != float(fieldset._time_s[0])))
-
-
-def _batch_levels(fieldset, d, evaluated) -> int:
-    """``pb_advect_args.batch_levels``: the reference's per-batch decisions a lane cannot make by itself.
-    PB_BATCH_FIRST_EVAL_TWO_T (1): see `_first_eval_two_levels`.  PB_BATCH_TWO_Z (2): `lenZ = 2 if any(zeta > 0)`
-    (_xinterpolators.py:401) -- with XFreeslip / XPartialslip the land test then looks at the second depth level for every particle
-    of the batch (:426-447); zeta > 0 means below the first depth level (left-sided search), taken as constant over the call."""
-    flags = 1 if _first_eval_two_levels(fieldset, d["t"], evaluated) else 0  # (`evaluated`: mask, or a callable making it on demand)
-    depth = fieldset.grid.depth
-    if fieldset.interp_method in ("freeslip", "partialslip") and depth is not None and len(depth) > 1:
-        ze = d["z"][evaluated() if callable(evaluated) else evaluated]
-        if ze.size and np.any(ze > depth[0]):
-            flags |= 2
-    return flags
-
-
-def _hint_all_zero(ei_last, evaluated, xdim) -> bool:
-    """Curvilinear grids: True when the hinted xi (= ei % xdim) of EVERY evaluated particle is 0 -- the reference then skips
-    the hint test for the whole batch (`if np.any(xi)`, _core/index_search.py:269).  `evaluated(slice)` gives the mask of a
-    slice of the set; a non-zero hint among the first few thousand particles settles the (usual) answer without a full pass."""
-    head = slice(0, min(len(ei_last), 4096))
-    if np.any((ei_last[head][evaluated(head)].astype(np.int64) % xdim) != 0):
-        return False
-    if not ei_last.any():  # a fresh set: every hint is 0 (one pass over the int32 column, no masked / widened copies)
-        return True
-    full = slice(None)
-    return not np.any((ei_last[evaluated(full)].astype(np.int64) % xdim) != 0)
-
-
-def _builtin_name(f):
-    """Name of the built-in kernel ``f`` stands for, or None for a user function.  Built-ins are this package's
-    tokens (kernels.py, by identity) and the reference package's own kernel functions (by module + name); a user
-    function that merely shares a name -- e.g. the ubiquitous user-defined ``DeleteParticle`` -- is NOT one."""
-    n = f.__name__
-    if n != "_none" and getattr(K, n, None) is f:
-        return n
-    mod = getattr(f, "__module__", "") or ""
-    if mod.startswith("parcels.kernels") and (n in K.SCHEMES or n in K.ADVDIFF or n in ("DiffusionUniformKh", "AdvectionRK45")) and n != "_none":
-        return n
+def _replay_first_error(plan, eng, rep, rewind, advance, dt, endtime):
+    """The reference stops the whole set at the END of the first loop iteration in which any particle is in an error state
+    (kernel.py:239-245): after a launch whose report ``rep`` saw one, ``rewind()`` to the start-of-interval copy and ``advance(k)``
+    (up to k loop iterations) again so that every particle is left exactly where the reference leaves it.  Returns the report
+    of the replay, or None when there is nothing to replay."""
+    k = rep["first_error_iter"]
+    if rep["n_error"] > 0:
+        rewind()
+        out = advance(k + 1)  # up to and including that iteration
+        if out["n_out_of_time"] > 0:
+            # an out-of-interval sample flags the WHOLE evaluated view (index_search.py:85-86, field.py:31-44)
+            rewind()
+            advance(k)
+            eng.flag_view_outside_time(dt, endtime)
+        return out
+    if plan.delete_on_error and rep["n_out_of_time"] > 0:
+        # Same whole-view rule under the DeleteParticle handler: every particle evaluated in the first iteration in which ANY
+        # particle sampled outside the time interval is flagged, hence deleted (field.py:31-44 then the handler) -- replay up
+        # to that iteration, then delete the view.  (The lanes deleted their own out-of-interval particle; the others ran on.)
+        rewind()
+        out = advance(k)
+        eng.delete_view_outside_time(dt, endtime)
+        out["n_deleted"] += 1
+        out["max_state"] = max(out["max_state"], int(StatusCode.Delete))
+        out["n_out_of_time"] = rep["n_out_of_time"]
+        return out
     return None
-
-
-def _delete_on_error(particles, fieldset):
-    """DeleteParticle token inside a stepwise list (reference idiom tests/common_kernels.py:12-13)."""
-    s = np.asarray(particles.state)
-    particles.state = np.where(s >= 50, StatusCode.Delete, s)
-
-
-def _assert_kernel_signature(f):
-    """A kernel function is ``f(particles, fieldset)`` (reference _python.py:33-52 `assert_same_function_signature` against
-    AdvectionRK4, called from Kernel.__init__, _core/kernel.py:69)."""
-    import inspect
-
-    params = list(inspect.signature(f).parameters.values())
-    if len(params) != 2:
-        raise ValueError(f"Kernel function must have 2 parameters, got {len(params)}")
-    for want, got in zip(("particles", "fieldset"), params, strict=True):
-        if got.kind != inspect.Parameter.POSITIONAL_OR_KEYWORD:
-            raise ValueError(f"Parameter '{got.name}' has incorrect parameter kind. Expected POSITIONAL_OR_KEYWORD, got {got.kind}")
-        if got.name != want:
-            raise ValueError(f"Parameter '{got.name}' has incorrect name. Expected '{want}', got '{got.name}'")
-
-
-class KernelPlan:
-    """The kernel list lowered to the fused device kernel's switches (include/parcels_b200.h)."""
-
-    def __init__(self, kernel_list, fieldset, pclass=None):
-        if isinstance(kernel_list, types.FunctionType):
-            kernel_list = [kernel_list]
-        if not isinstance(kernel_list, list):
-            raise ValueError(f"kernels must be a list. Got {kernel_list=!r}")
-        if len(kernel_list) == 0:
-            raise ValueError("List of `kernels` should have at least one function.")
-        for f in kernel_list:
-            if not isinstance(f, types.FunctionType):
-                raise TypeError(f"Argument `kernels` should be a function or list of functions. Got {type(f)}")
-            _assert_kernel_signature(f)
-        self.funcname = "".join(f.__name__ for f in kernel_list)
-        tokens = [_builtin_name(f) for f in kernel_list]  # None for user functions (recognised by identity, not by name)
-        names = list(tokens)
-        self.delete_on_error = self.diffusion = False
-        if names and names[-1] == "DeleteParticle":
-            self.delete_on_error = True
-            names = names[:-1]
-        if names and names[-1] == "DiffusionUniformKh":
-            self.diffusion = True
-            names = names[:-1]
-        if len(names) == 0 and self.diffusion:
-            names = ["_none"]
-        self.rk45 = None
-        self.advdiff = None
-        self._kernel_list, self._tokens = kernel_list, tokens
-        if "AdvectionRK45" in tokens:
-            self._setup_rk45(names, fieldset, pclass)
-            return
-        if len(names) == 1 and names[0] in K.ADVDIFF and not self.diffusion:
-            self._setup_advdiff(names, fieldset)  # [kernel] or [kernel, DeleteParticle]: the whole loop in one launch
-            return
-        if "DiffusionUniformKh" in tokens and any(n in K.ADVDIFF for n in tokens if n):
-            raise NotImplementedError("AdvectionDiffusionM1/EM already diffuse: combining them with DiffusionUniformKh is not supported")
-        self.stepwise = not (len(names) == 1 and names[0] in K.SCHEMES)
-        if fieldset.time_window is not None and not self.delete_on_error:
-            # without the DeleteParticle token an error must stop the whole set at the end of its iteration; the fused kernel
-            # could only replay that iteration from the start of the interval, whose time levels the window has left behind
-            self.stepwise = True
-        if self.stepwise:
-            # the list mixes built-ins with user Python kernels: the loop control runs on the host step by step
-            # (stepwise.py), every built-in kernel still runs on the device
-            self.delete_on_error = self.diffusion = False
-            self.items = []
-            for f, n in zip(kernel_list, tokens, strict=True):
-                if n in K.SCHEMES:
-                    if n in K.SCHEMES_3D and fieldset.W is None:
-                        raise AttributeError("FieldSet has no UVW VectorField (no W field) for a 3-D advection kernel")
-                    self.items.append(["device", K.SCHEMES[n], False, self])
-                elif n == "DiffusionUniformKh":
-                    if self.items and self.items[-1][0] == "device" and not self.items[-1][2]:
-                        self.items[-1][2] = True  # fused with the advection kernel right before it
-                    else:
-                        self.items.append(["device", K.SCHEMES["_none"], True, self])
-                elif n in K.ADVDIFF:  # mixed with user kernels: one device launch per step (kernels_only)
-                    self.items.append(["advdiff", _advdiff_params(fieldset, n)])
-                elif n == "DeleteParticle":
-                    self.items.append(["python", _delete_on_error])
-                else:
-                    self.items.append(["python", f])
-            self.scheme_name, self.scheme = "stepwise", -1
-        else:
-            self.scheme_name = names[0]
-            self.scheme = K.SCHEMES[names[0]]
-            if names[0] in K.SCHEMES_3D and fieldset.W is None:
-                raise AttributeError("FieldSet has no UVW VectorField (no W field) for a 3-D advection kernel")
-        self.kh = (0.0, 0.0)
-        self.kh_spherical = False
-        self.kh_deg2m = 1.0
-        if self.diffusion or (self.stepwise and any(i[0] == "device" and i[2] for i in self.items)):
-            try:
-                self.kh = (fieldset.constants["Kh_zonal"], fieldset.constants["Kh_meridional"])
-            except KeyError as e:
-                raise AttributeError("DiffusionUniformKh needs constant fields Kh_zonal and Kh_meridional") from e
-            g = fieldset.Kh_zonal.grid
-            self.kh_spherical = g.is_spherical()
-            self.kh_deg2m = g.deg2m
-
-
-def _setup_rk45(self, names, fieldset, pclass):
-    """AdvectionRK45 (reference _core/kernel.py:134-159 `check_fieldsets_in_kernels`): needs a `next_dt` Variable; missing
-    RK45_tol / RK45_min_dt / RK45_max_dt get the reference's defaults with a KernelWarning; on a spherical mesh the
-    tolerance is converted to degrees -- like the reference, in place, every time a kernel list is built."""
-    import warnings
-
-    from .statuscodes import KernelWarning
-
-    fused = names == ["AdvectionRK45"] and not self.diffusion
-    if self.diffusion or any(n in K.SCHEMES or n in K.ADVDIFF or n == "DiffusionUniformKh" for n in names if n):
-        raise NotImplementedError("AdvectionRK45 combines with user kernels and the DeleteParticle token, not with other built-in kernels")
-    if pclass is None or "next_dt" not in [v.name for v in pclass.variables]:
-        raise ValueError('ParticleClass requires a "next_dt" for AdvectionRK45 Kernel.')
-    if not ((fieldset.interp_method in ("linear", "freeslip", "partialslip") and not fieldset.grid.curvilinear)
-            or fieldset.interp_method == "cgrid_velocity"):  # fmt: skip
-        raise NotImplementedError("AdvectionRK45 is implemented for XLinear_Velocity, XFreeslip or XPartialslip "
-                                  "(rectilinear A-grids) or CGrid_Velocity (rectilinear and curvilinear C-grids)")
-    ctx = fieldset.context
-    if "RK45_tol" not in ctx:
-        warnings.warn("Setting RK45 tolerance to 10 m. Use fieldset.add_context('RK45_tol', [distance]) to change.", KernelWarning, stacklevel=4)
-        fieldset.add_context("RK45_tol", 10)
-    if fieldset.grid.is_spherical() and not getattr(fieldset, "_context_is_reference", False):
-        # (under parcels_b200.install() the context mirrors the reference FieldSet's, whose own Kernel.__init__ has converted it)
-        ctx["RK45_tol"] = ctx["RK45_tol"] / fieldset.grid.deg2m
-    if "RK45_min_dt" not in ctx:
-        warnings.warn("Setting RK45 minimum timestep to 1 s. Use fieldset.add_context('RK45_min_dt', [timestep]) to change.", KernelWarning, stacklevel=4)
-        fieldset.add_context("RK45_min_dt", 1)
-    if "RK45_max_dt" not in ctx:
-        warnings.warn("Setting RK45 maximum timestep to 1 day. Use fieldset.add_context('RK45_max_dt', [timestep]) to change.", KernelWarning, stacklevel=4)
-        fieldset.add_context("RK45_max_dt", 60 * 60 * 24)
-    self.rk45 = (float(ctx["RK45_tol"]), float(ctx["RK45_min_dt"]), float(ctx["RK45_max_dt"]))
-    self.kh, self.kh_spherical, self.kh_deg2m = (0.0, 0.0), False, 1.0
-    if fused:  # [AdvectionRK45] or [AdvectionRK45, DeleteParticle]: the whole loop in one launch
-        self.stepwise = False
-        self.scheme_name, self.scheme = "AdvectionRK45", K.RK45
-        return
-    # mixed with user kernels (the reference's own tests/test_advection.py:354-387: [AdvectionRK45, UpdateP]): the host drives the
-    # loop, every iteration's RK45 attempts run on the device (pb_advect_rk45 with kernels_only)
-    self.stepwise = True
-    self.scheme_name, self.scheme = "stepwise", -1
-    self.delete_on_error = False
-    self.items = []
-    for f, n in zip(self._kernel_list, self._tokens, strict=True):
-        if n == "AdvectionRK45":
-            self.items.append(["rk45", self.rk45])
-        elif n == "DeleteParticle":
-            self.items.append(["python", _delete_on_error])
-        else:
-            self.items.append(["python", f])
-    self.rk45 = None  # (fused-path marker)
-
-
-KernelPlan._setup_rk45 = _setup_rk45
-
-
-def _advdiff_params(fieldset, name):
-    """AdvectionDiffusionM1 / AdvectionDiffusionEM (reference kernels/_advectiondiffusion.py:21-117): need the scalar fields
-    ``Kh_zonal`` / ``Kh_meridional`` on the fieldset's grid and the context value ``dres`` -> arguments of pb_advect_diffusion."""
-    from .fieldset import Field
-
-    kz, km = fieldset.fields.get("Kh_zonal"), fieldset.fields.get("Kh_meridional")
-    if not isinstance(kz, Field) or not isinstance(km, Field):
-        raise AttributeError(f"{name} needs fields Kh_zonal and Kh_meridional (FieldSet.add_field)")
-    if kz._slot is None or km._slot is None or kz.interp_method != "linear" or km.interp_method != "linear":
-        raise NotImplementedError(f"{name}: Kh_zonal / Kh_meridional must be XLinear scalar fields on the FieldSet's grid "
-                                  "(FieldSet.add_field(name, data)); constant fields have no gradient -- use DiffusionUniformKh")  # fmt: skip
-    if fieldset.grid.curvilinear or fieldset.interp_method not in ("linear", "cgrid_velocity"):
-        raise NotImplementedError(f"{name} is implemented for rectilinear fields (XLinear_Velocity or CGrid_Velocity)")
-    if kz.data.dtype != km.data.dtype or (kz.data.shape[0] > 1) != (km.data.shape[0] > 1):
-        raise NotImplementedError("Kh_zonal and Kh_meridional must share dtype and time dimension")
-    if "dres" not in fieldset.context:
-        raise AttributeError(f"{name} needs fieldset.add_context('dres', <resolution of the Kh gradient>)")
-    dres = fieldset.context["dres"]
-    if isinstance(dres, np.generic) or not isinstance(dres, (int, float)):
-        # a NumPy float64 scalar is a STRONG type: `particles.x + dres` would be a float64 array in the reference and the
-        # whole kernel would run in other dtypes; the reference's own usage passes a Python float (tests/test_diffusion.py:65)
-        raise NotImplementedError("fieldset.dres must be a Python float (fieldset.add_context('dres', float(...)))")
-    return dict(scheme=K.ADVDIFF[name], kh_slots=(kz._slot, km._slot), dres=float(dres), deg2m_sq=pow(fieldset.grid.deg2m, 2))
-
-
-def _setup_advdiff(self, names, fieldset):
-    self.advdiff = _advdiff_params(fieldset, names[0])
-    self.stepwise = False
-    self.scheme_name, self.scheme = names[0], -2
-    self.kh, self.kh_spherical, self.kh_deg2m = (0.0, 0.0), False, 1.0
-
-
-KernelPlan._setup_advdiff = _setup_advdiff
 
 
 class Kernel:
@@ -393,14 +167,8 @@ class Kernel:
     ``(particles, fieldset)`` signature, RK45 prerequisites) and names it; ``pset.execute`` lowers the same list to device launches."""
 
     def __init__(self, kernels, pset):
-        if not isinstance(kernels, list):
+        if not isinstance(kernels, list):  # (KernelPlan also takes a bare function)
             raise ValueError(f"kernels must be a list. Got {kernels=!r}")
-        for f in kernels:
-            if not isinstance(f, types.FunctionType):
-                raise TypeError(f"Argument `kernels` should be a function or list of functions. Got {type(f)}")
-            _assert_kernel_signature(f)
-        if len(kernels) == 0:
-            raise ValueError("List of `kernels` should have at least one function.")
         self._fieldset = pset.fieldset
         self._pclass = pset._pclass
         self._plan = KernelPlan(kernels, pset.fieldset, pset._pclass)
@@ -532,7 +300,7 @@ class ParticleSet:
         """Can the set stay device-resident across output intervals?  Built-in kernel lists on rectilinear grids with
         the default Particle variables (extra variables live on the host; the curvilinear hint test needs host `ei`)."""
         fs = self.fieldset
-        return not plan.stepwise and plan.rk45 is None and not fs.grid.curvilinear and fs.time_window is None and len(self._pclass.extra) == 0
+        return plan.kind in ("fixed", "advdiff") and not fs.grid.curvilinear and fs.time_window is None and len(self._pclass.extra) == 0
 
     def _output_columns(self, t, names, indices=None):
         """Rows due for output at time ``t`` (reference `_to_write_particles`, _core/particlefile.py:198-221) of the
@@ -676,7 +444,7 @@ class ParticleSet:
                 raise ValueError("Time values cannot be NaN.")
             self._device_synced = False
             return kernel_execute_stepwise(self, plan, endtime, dt)
-        if plan.rk45 is not None:
+        if plan.kind == "rk45":
             return self._kernel_execute_rk45(plan, endtime, dt)
         eng = self.fieldset.engine(self.device)
         eng.claim(self)  # a ParticleSet that was resident here is synced to its host arrays first
@@ -700,39 +468,25 @@ class ParticleSet:
                 raise ValueError(f"Time values for particles with indices {bad} cannot be NaN.")  # field.py:396-398
             ei_last = _ei_last(d, self)
         self._rng_call += 1
-        hint_all_zero = False
-        g = self.fieldset.grid
-        if g.curvilinear:
-            # the reference skips the hint test for the WHOLE batch when every hinted xi is 0
-            # (`if np.any(xi)`, _core/index_search.py:269), e.g. on the first eval of a fresh set
-            sign = 1 if dt > 0 else -1
-            hint_all_zero = _hint_all_zero(ei_last, lambda s_: sign * (endtime - d["t"][s_]) >= 0, g.xdim)
-
         if on_device:  # a resident interval: no particle can be back on the first time level; the depth bit of the first interval holds
-            two_levels = self.__dict__.get("_batch_levels_resident", 0) & 2
+            hint_all_zero, two_levels = False, self.__dict__.get("_batch_levels_resident", 0) & 2
         else:
-            two_levels = _batch_levels(self.fieldset, d, lambda: (1 if dt > 0 else -1) * (endtime - d["t"]) >= 0)
+            # (curvilinear grids: the reference skips the hint test for the WHOLE batch when every hinted xi is 0, e.g. on the first
+            # eval of a fresh set)
+            hint_all_zero, two_levels = batch_facts(self.fieldset, d, ei_last, dt, endtime)
             self.__dict__["_batch_levels_resident"] = two_levels
 
-        def args(max_iters=-1):
-            if plan.advdiff is not None:
-                return eng.make_advdiff_args(dt=dt, endtime=endtime, delete_on_error=plan.delete_on_error, seed=self.seed,
-                                             rng_call=self._rng_call, max_iters=max_iters, batch_levels=two_levels,
-                                             **plan.advdiff)  # fmt: skip
-            return eng.make_args(plan.scheme, dt, endtime, diffusion=plan.diffusion, delete_on_error=plan.delete_on_error,
-                                 kh=plan.kh, kh_spherical=plan.kh_spherical, kh_deg2m=plan.kh_deg2m, seed=self.seed,
-                                 rng_call=self._rng_call, max_iters=max_iters, hint_all_zero=hint_all_zero,
-                                 batch_levels=two_levels)  # fmt: skip
+        def args(max_iters=-1, resume=False):
+            return plan.launch_args(eng, dt, endtime, seed=self.seed, rng_call=self._rng_call, max_iters=max_iters, resume=resume,
+                                    hint_all_zero=hint_all_zero, batch_levels=two_levels)  # fmt: skip
 
         needs_upload = not on_device and not (resident and self._device_synced and eng.particle_count() == n)
-        if not on_device and self.__dict__.get("_dt_pending") is not None and not (
-                needs_upload and self.pipeline_chunks > 1 and n >= self.PIPELINE_MIN_PARTICLES and plan.advdiff is None
-                and self.fieldset.time_window is None):  # fmt: skip
+        # host arrays in (and out): cut into chunks whose copies run under the kernels of the other chunks (pb_advect_host)
+        pipelined = (needs_upload and self.pipeline_chunks > 1 and n >= self.PIPELINE_MIN_PARTICLES and plan.kind == "fixed"
+                     and self.fieldset.time_window is None)  # fmt: skip
+        if not on_device and not pipelined and self.__dict__.get("_dt_pending") is not None:
             _fill(d["dt"], self.__dict__.pop("_dt_pending"))  # (not the pipelined path: the deferred fill is done here)
             self.__dict__["_dt_filled"] = (d["dt"], dt)
-        # host arrays in (and out): cut into chunks whose copies run under the kernels of the other chunks (pb_advect_host)
-        pipelined = (needs_upload and self.pipeline_chunks > 1 and n >= self.PIPELINE_MIN_PARTICLES and plan.advdiff is None
-                     and self.fieldset.time_window is None)  # fmt: skip
         downloaded = False
         if needs_upload and not pipelined:
             eng.upload_particles(d, ei_last)
@@ -756,14 +510,12 @@ class ParticleSet:
                     # advect_kernel restarts its iteration count, so it gets its own call index -- otherwise the same increments
                     # would be drawn again.  (pb_advect_diffusion continues each particle's count: its stream needs no new index.)
                     self._rng_call += 1
-                a = args(max_iters=max_iters)
-                a.resume = int(resume)
-                eng.advect_async(a)
+                eng.advect_async(args(max_iters=max_iters, resume=resume))
 
             return self._advect_windowed(eng, d, dt, endtime, launch)
 
         # pb_advect_diffusion counts the iterations of a windowed call across its launches: its replay is exact as well
-        replayable = not windowed or plan.advdiff is not None
+        replayable = not windowed or plan.kind == "advdiff"
         if windowed:
             rep = advance()
         elif pipelined:
@@ -783,32 +535,9 @@ class ParticleSet:
                     filler.join()
         else:
             rep = advance()
-        if rep["n_error"] > 0 and replayable:
-            # The reference stops the whole set at the END of the first loop iteration in which any
-            # particle is in an error state (kernel.py:239-245).  Replay from the start-of-interval copy up to
-            # and including that iteration so every particle is left exactly where the reference leaves it.
-            k = rep["first_error_iter"]
-            rewind()
-            downloaded = False
-            rep = advance(k + 1)
-            if rep["n_out_of_time"] > 0:
-                # an out-of-interval sample flags the WHOLE evaluated view (index_search.py:85-86, field.py:31-44)
-                rewind()
-                advance(k)
-                eng.flag_view_outside_time(dt, endtime)
-        elif plan.delete_on_error and rep["n_out_of_time"] > 0 and replayable:
-            # Same whole-view rule under the DeleteParticle handler: every particle evaluated in the first iteration in which ANY
-            # particle sampled outside the time interval is flagged, hence deleted (field.py:31-44 then the handler) -- replay up
-            # to that iteration, then delete the view.  (The lanes deleted their own out-of-interval particle; the others ran on.)
-            k = rep["first_error_iter"]
-            rewind()
-            downloaded = False
-            first = rep
-            rep = advance(k)
-            eng.delete_view_outside_time(dt, endtime)
-            rep["n_deleted"] += 1
-            rep["max_state"] = max(rep["max_state"], int(StatusCode.Delete))
-            rep["n_out_of_time"] = first["n_out_of_time"]
+        replayed = _replay_first_error(plan, eng, rep, rewind, advance, dt, endtime) if replayable else None
+        if replayed is not None:
+            rep, downloaded = replayed, False
         self.last_report = rep
         self._stale_dt = dt
         if lazy and rep["max_state"] < StatusCode.Error:
@@ -864,49 +593,59 @@ class ParticleSet:
         """``Kernel.execute`` with AdvectionRK45 (reference _core/kernel.py:108-120,190-245): per-particle dt / next_dt,
         Repeat loop and step doubling run inside ONE device kernel (csrc/rk45.cu); dt is not reset to the nominal step."""
         d = self._data
-        n = len(self)
         self._device_synced = False
         d["state"][:] = StatusCode.Evaluate
-        if n == 0:
+        if len(self) == 0:
             return
         if np.isnan(d["t"]).any():
             raise ValueError(f"Time values for particles with indices {np.where(np.isnan(d['t']))[0]} cannot be NaN.")
         eng = self.fieldset.engine(self.device)
         eng.claim(self)
-        ei_last = np.ascontiguousarray(d["ei"][:, -1])
-        eng.upload_particles(d, ei_last)
-        dt_arr = np.ascontiguousarray(d["dt"], dtype=np.float64)
-        ndt_arr = np.ascontiguousarray(d["next_dt"], dtype=np.float64)
-        tol, min_dt, max_dt = plan.rk45
-        hint_all_zero = False
-        if self.fieldset.grid.curvilinear:  # batch-level `if np.any(xi)` of the first evaluation (index_search.py:269)
-            sign = 1 if dt > 0 else -1
-            hint_all_zero = _hint_all_zero(ei_last, lambda s_: sign * (endtime - d["t"][s_]) >= 0, self.fieldset.grid.xdim)
-        two_levels = _batch_levels(self.fieldset, d, lambda: (1 if dt > 0 else -1) * (endtime - d["t"]) >= 0)
-
-        def launch(resume):  # (a resumed launch continues every particle's dt, next_dt and iteration count)
-            return eng.advect_rk45(dt, endtime, tol, min_dt, max_dt, dt_arr, ndt_arr, next_dt_is_f32=d["next_dt"].dtype == np.float32,
-                                   delete_on_error=plan.delete_on_error, hint_all_zero=hint_all_zero, batch_levels=two_levels,
-                                   resume=resume)  # fmt: skip
-
-        if self.fieldset.time_window is not None:
-            rep = self._advect_windowed(eng, d, dt, endtime, launch, synchronous=True)
-        else:
-            rep = launch(False)
-        self.last_report = rep
-        eng.download_particles(d, ei_last)
-        _store_ei(d, ei_last)
-        d["dt"][:] = dt_arr  # RK45 mode: dt is NOT reset to the nominal step (kernel.py:224-226)
-        d["next_dt"][:] = ndt_arr
-        if rep["n_error"] > 0:
-            stuck = np.where(d["state"] == StatusCode.Error)[0]
-            raise RuntimeError(f"AdvectionRK45: particles {stuck[:10]} have dt == 0 before endtime={endtime}; the reference's loop "
-                               "never terminates on them (kernel.py:199-203 clamps the dt of particles that finished an earlier "
-                               "interval to 0 and RK45 mode never restores it).  Reset pset.dt before continuing.")  # fmt: skip
+        rep = self._advect_rk45(plan, eng, dt, endtime)
         if rep["max_state"] == StatusCode.Delete:
             dele = np.where(d["state"] == StatusCode.Delete)[0]
             if len(dele) > 0:
                 self.remove_indices(dele)
+
+    def _advect_rk45(self, plan, eng, dt, endtime, *, stepwise=False):
+        """Upload, AdvectionRK45 on the device (pb_advect_rk45) and write-back of positions, states, ``ei``, dt and next_dt (the
+        reference leaves every particle's own dt: it is not reset to the nominal step, kernel.py:224-226).  ``stepwise``: ONE
+        iteration of a stepwise list (kernels_only) -- every evaluated particle's attempts until its step is accepted, the
+        reference's `while state == Repeat` re-runs of the kernel (kernel.py:212-216); the host does the position update.
+        Otherwise the whole loop of the call, through the time window's levels on a time-windowed FieldSet."""
+        d = self._data
+        ei_last = np.ascontiguousarray(d["ei"][:, -1])
+        eng.upload_particles(d, ei_last)
+        dt_arr = np.ascontiguousarray(d["dt"], dtype=np.float64)
+        ndt_arr = np.ascontiguousarray(d["next_dt"], dtype=np.float64)
+        hint_all_zero, two_levels = batch_facts(self.fieldset, d, ei_last, dt, endtime, mid_iteration=stepwise)
+
+        def launch(resume):  # (a resumed launch continues every particle's dt, next_dt and iteration count)
+            args = plan.launch_args(eng, dt, endtime, hint_all_zero=hint_all_zero, batch_levels=two_levels, resume=resume,
+                                    kernels_only=stepwise, next_dt_dtype=d["next_dt"].dtype)  # fmt: skip
+            return eng.advect_rk45(args, dt_arr, ndt_arr)
+
+        if stepwise:
+            from .stepwise import _no_wait
+
+            rep = launch(True)
+            _no_wait(rep)
+        elif self.fieldset.time_window is None:
+            rep = self.last_report = launch(False)
+        else:
+            rep = self.last_report = self._advect_windowed(eng, d, dt, endtime, launch, synchronous=True)
+        eng.download_particles(d, ei_last)
+        _store_ei(d, ei_last)
+        d["dt"][:] = dt_arr
+        d["next_dt"][:] = ndt_arr
+        if rep["n_error"] > 0:
+            stuck = np.where(d["state"] == StatusCode.Error)[0]
+            if stepwise:
+                raise RuntimeError(f"AdvectionRK45: particles {stuck[:10]} have dt == 0 before endtime={endtime}; reset pset.dt before continuing")
+            raise RuntimeError(f"AdvectionRK45: particles {stuck[:10]} have dt == 0 before endtime={endtime}; the reference's loop "
+                               "never terminates on them (kernel.py:199-203 clamps the dt of particles that finished an earlier "
+                               "interval to 0 and RK45 mode never restores it).  Reset pset.dt before continuing.")  # fmt: skip
+        return rep
 
     def _advect_windowed(self, eng, d, dt, endtime, launch, *, synchronous=False):
         """Time-slab streaming: advance until every particle reached ``endtime``, sliding the resident time levels as the
@@ -916,7 +655,7 @@ class ParticleSet:
         back) returns its report; the next level is copied before it, under the kernel only when the level data is pinned."""
         fs = self.fieldset
         sign = 1 if dt > 0 else -1
-        todo = sign * (endtime - d["t"]) >= 0
+        todo = evaluated_mask(d, dt, endtime)
         t_ref = (d["t"][todo].min() if sign > 0 else d["t"][todo].max()) if todo.any() else float(d["t"][0])
         fs.slide_window(self.device, t_ref, sign)
         total = None
@@ -960,7 +699,7 @@ class ParticleSet:
         # 80 MB pass per 1e7 particles is taken off the critical path: a large set's column is filled by a helper thread WHILE the first
         # pipelined Kernel.execute runs on the GPU (`_dt_pending` -> `_kernel_execute`); `_fill_dt` need not write it again at the end
         # (`_dt_filled`).  Plans with user kernels or RK45 read / write per-particle steps: filled here, no mark.
-        fused = not plan.stepwise and plan.rk45 is None
+        fused = plan.kind in ("fixed", "advdiff")
         if fused and len(self) >= self.PIPELINE_MIN_PARTICLES and not self._host_stale:
             self.__dict__["_dt_pending"] = dt
         else:

@@ -18,6 +18,7 @@ from __future__ import annotations
 import numpy as np
 
 from .particlesetview import ParticleSetView
+from .plan import PythonStep, Rk45Step, batch_facts
 from .statuscodes import ERRORS_TO_THROW, StatusCode, raise_for_state
 
 
@@ -40,15 +41,15 @@ def kernel_execute_stepwise(pset, plan, endtime: float, dt: float):
         # adapt dt to end exactly on endtime (kernel.py:199-203)
         d["dt"][:] = np.maximum(np.minimum(d["dt"], tte), 0) if sign == 1 else np.minimum(np.maximum(d["dt"], -tte), 0)
         steps += int(np.count_nonzero(evaluate))
-        for item in plan.items:
-            if item[0] != "python" and fs.time_window is not None:
+        for step in plan.items:
+            if not isinstance(step, PythonStep) and fs.time_window is not None:
                 _cover_steps(pset, evaluate, sign)
-            if item[0] in ("device", "advdiff"):
-                _device_kernels(pset, eng, item, dt, endtime)
-            elif item[0] == "rk45":
-                _device_rk45(pset, eng, item[1], dt, endtime)
+            if isinstance(step, Rk45Step):
+                pset._advect_rk45(plan, eng, dt, endtime, stepwise=True)
+            elif not isinstance(step, PythonStep):
+                _device_kernels(pset, eng, plan, step, dt, endtime)
             else:
-                f = item[1]
+                f = step.func
                 f(ParticleSetView(d, evaluate, fs), fs)
                 repeat = d["state"] == StatusCode.Repeat
                 while np.any(repeat):  # kernel.py:213-216
@@ -101,38 +102,17 @@ def _no_wait(rep):
         raise RuntimeError(f"{rep['n_wait_window']} particles found their time levels not resident: widen time_window")
 
 
-def _device_kernels(pset, eng, item, dt, endtime):
-    """One iteration of the built-in kernels ``item`` on the device: the kernel applies the reference's own
-    evaluate mask (state in {Success, Evaluate} and time-to-endtime >= 0) and dt clamp, accumulates dx/dy/dz and
-    updates state/ei; nothing else."""
+def _device_kernels(pset, eng, plan, step, dt, endtime):
+    """One iteration of the built-in kernels ``step`` (a FixedStep or an AdvDiffStep of ``plan``) on the device: the kernel
+    applies the reference's own evaluate mask (state in {Success, Evaluate} and time-to-endtime >= 0) and dt clamp, accumulates
+    dx/dy/dz and updates state/ei; nothing else."""
     d = pset._data
     pset._rng_call += 1
     ei_last = np.ascontiguousarray(d["ei"][:, -1])
-    hint_all_zero = False
-    g = pset.fieldset.grid
-    if g.curvilinear:
-        from .particleset import _hint_all_zero
-
-        sign = 1 if dt > 0 else -1
-        hint_all_zero = _hint_all_zero(
-            ei_last, lambda s_: np.isin(d["state"][s_], [StatusCode.Success, StatusCode.Evaluate]) & (sign * (endtime - d["t"][s_]) >= 0), g.xdim
-        )
+    hint_all_zero, two_levels = batch_facts(pset.fieldset, d, ei_last, dt, endtime, mid_iteration=True)
     eng.upload_particles(d, ei_last)
-    from .particleset import _batch_levels
-
-    sign_ = 1 if dt > 0 else -1
-    two_levels = _batch_levels(
-        pset.fieldset, d, lambda: np.isin(d["state"], [StatusCode.Success, StatusCode.Evaluate]) & (sign_ * (endtime - d["t"]) >= 0)
-    )
-    if item[0] == "advdiff":  # AdvectionDiffusionM1 / EM (pb_advect_diffusion)
-        args = eng.make_advdiff_args(dt=dt, endtime=endtime, seed=pset.seed, rng_call=pset._rng_call, resume=True, kernels_only=True,
-                                     batch_levels=two_levels, **item[1])  # fmt: skip
-    else:
-        _, scheme, diffusion, plan = item
-        args = eng.make_args(scheme, dt, endtime, diffusion=diffusion, kh=plan.kh, kh_spherical=plan.kh_spherical,
-                             kh_deg2m=plan.kh_deg2m, seed=pset.seed, rng_call=pset._rng_call, hint_all_zero=hint_all_zero,
-                             resume=True, kernels_only=True, batch_levels=two_levels)  # fmt: skip
-    rep = eng.advect(args)
+    rep = eng.advect(plan.launch_args(eng, dt, endtime, step=step, seed=pset.seed, rng_call=pset._rng_call, hint_all_zero=hint_all_zero,
+                                      batch_levels=two_levels, resume=True, kernels_only=True))  # fmt: skip
     _no_wait(rep)
     eng.download_particles(d, ei_last)
     d["ei"][:, -1] = ei_last
@@ -142,40 +122,3 @@ def _device_kernels(pset, eng, item, dt, endtime):
             sign * (endtime - d["t"]) >= 0
         )
         d["state"][view] = StatusCode.ErrorOutsideTimeInterval
-
-
-def _device_rk45(pset, eng, params, dt, endtime):
-    """One iteration of AdvectionRK45 on the device (``pb_advect_rk45`` with kernels_only): every evaluated particle's attempts until
-    its step is accepted -- the reference's `while state == Repeat` re-runs of the kernel (kernel.py:212-216) -- with dx / dy,
-    dt, next_dt, state and ei written back; the host does the position update and `dt <- next_dt`."""
-    d = pset._data
-    ei_last = np.ascontiguousarray(d["ei"][:, -1])
-    eng.upload_particles(d, ei_last)
-    dt_arr = np.ascontiguousarray(d["dt"], dtype=np.float64)
-    ndt_arr = np.ascontiguousarray(d["next_dt"], dtype=np.float64)
-    tol, min_dt, max_dt = params
-    hint_all_zero = False
-    g = pset.fieldset.grid
-    if g.curvilinear:
-        from .particleset import _hint_all_zero
-
-        sign = 1 if dt > 0 else -1
-        hint_all_zero = _hint_all_zero(
-            ei_last, lambda s_: np.isin(d["state"][s_], [StatusCode.Success, StatusCode.Evaluate]) & (sign * (endtime - d["t"][s_]) >= 0), g.xdim
-        )
-    from .particleset import _batch_levels
-
-    sign_ = 1 if dt > 0 else -1
-    two_levels = _batch_levels(
-        pset.fieldset, d, lambda: np.isin(d["state"], [StatusCode.Success, StatusCode.Evaluate]) & (sign_ * (endtime - d["t"]) >= 0)
-    )
-    rep = eng.advect_rk45(dt, endtime, tol, min_dt, max_dt, dt_arr, ndt_arr, next_dt_is_f32=d["next_dt"].dtype == np.float32,
-                          kernels_only=True, resume=True, hint_all_zero=hint_all_zero, batch_levels=two_levels)  # fmt: skip
-    _no_wait(rep)
-    eng.download_particles(d, ei_last)
-    d["ei"][:, -1] = ei_last
-    d["dt"][:] = dt_arr
-    d["next_dt"][:] = ndt_arr
-    if rep["n_error"] > 0:
-        stuck = np.where(d["state"] == StatusCode.Error)[0]
-        raise RuntimeError(f"AdvectionRK45: particles {stuck[:10]} have dt == 0 before endtime={endtime}; reset pset.dt before continuing")

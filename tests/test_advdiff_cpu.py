@@ -40,7 +40,7 @@ def test_advdiff_plan_checks():
 
     plan = KernelPlan([pb.AdvectionDiffusionM1, pb.DeleteParticle], _fieldset())
     assert plan.advdiff == dict(scheme=0, kh_slots=(3, 4), dres=0.5, deg2m_sq=pow(_fieldset().grid.deg2m, 2))
-    assert plan.delete_on_error and not plan.stepwise
+    assert plan.kind == "advdiff" and plan.delete_on_error and not plan.stepwise
     assert KernelPlan([pb.AdvectionDiffusionEM], _fieldset()).advdiff["scheme"] == 1
     with pytest.raises(AttributeError, match="Kh_zonal"):
         KernelPlan([pb.AdvectionDiffusionM1], _fieldset(with_kh=False))

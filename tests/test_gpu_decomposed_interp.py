@@ -126,4 +126,4 @@ def test_refusals():
     for interp in ("cgrid", "freeslip", "partialslip"):
         case = decomposed_kernels.make_case("rk45", n=10, interp=interp)
         plan = D.decomposed_plan(decomposed_kernels.decomposed_fieldset(case, 1, 2), case["kernels"], case["full"])
-        assert plan.rk45 is not None
+        assert plan.kind == "rk45" and plan.rk45 is not None

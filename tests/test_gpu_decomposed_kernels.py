@@ -97,4 +97,4 @@ def test_refusals():
     with pytest.raises(NotImplementedError, match="one built-in kernel"):
         D.decomposed_plan(dfs, [pb.AdvectionRK45, user, pb.DeleteParticle], case["full"])
     plan = D.decomposed_plan(dfs, case["kernels"], case["full"])
-    assert plan.rk45 is not None and plan.next_dt_dtype == np.float32
+    assert plan.kind == "rk45" and plan.rk45 is not None and plan.next_dt_dtype == np.float32

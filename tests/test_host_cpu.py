@@ -11,6 +11,7 @@ import pytest
 import parcels_b200 as pb
 from parcels_b200 import _lib
 from parcels_b200.particleset import KernelPlan
+from parcels_b200.plan import FixedStep, PythonStep
 from philox_ref import philox4x32_10, wiener_normals
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -53,7 +54,7 @@ def _fs(with_w=True):
 def test_kernel_plan_lowering():
     fs = _fs()
     p = KernelPlan([pb.AdvectionRK4_3D, pb.DeleteParticle], fs)
-    assert (p.scheme, p.diffusion, p.delete_on_error) == (5, False, True)
+    assert (p.kind, p.scheme, p.diffusion, p.delete_on_error) == ("fixed", 5, False, True)
     fs.add_constant_field("Kh_zonal", 100, mesh="flat")
     fs.add_constant_field("Kh_meridional", 50, mesh="flat")
     p = KernelPlan([pb.AdvectionRK4, pb.DiffusionUniformKh], fs)
@@ -61,7 +62,7 @@ def test_kernel_plan_lowering():
     assert len(fs.gridset) == 2  # constant fields live on their own grid => ei has 2 columns
 
 
-def test_kernel_plan_mixed_lists_keep_builtins_on_the_device():
+def test_kernel_plan_mixed_lists_lower_to_step_records_with_builtins_on_the_device():
     def MyKernel(particles, fieldset):
         pass
 
@@ -72,9 +73,13 @@ def test_kernel_plan_mixed_lists_keep_builtins_on_the_device():
     fs.add_constant_field("Kh_zonal", 1.0, mesh="flat")
     fs.add_constant_field("Kh_meridional", 1.0, mesh="flat")
     p = KernelPlan([pb.AdvectionRK4, pb.DiffusionUniformKh, MyKernel, DeleteParticle], fs)
-    assert p.stepwise and [i[0] for i in p.items] == ["device", "python", "python"]
-    assert p.items[0][1:3] == [4, True]  # AdvectionRK4 fused with DiffusionUniformKh in one device call
-    assert p.items[2][1] is DeleteParticle
+    assert p.kind == "stepwise" and p.stepwise and [type(s) for s in p.items] == [FixedStep, PythonStep, PythonStep]
+    assert p.items[0] == FixedStep(scheme=4, diffusion=True)  # AdvectionRK4 fused with DiffusionUniformKh in one device call
+    assert p.items[2].func is DeleteParticle
+    with pytest.raises(AttributeError):  # the records are immutable: fusing replaces the step, it never edits one
+        p.items[0].diffusion = False
+    alone = KernelPlan([MyKernel, pb.DiffusionUniformKh, MyKernel], fs)  # no advection step to fuse with: diffusion on its own
+    assert alone.items == (PythonStep(MyKernel), FixedStep(scheme=0, diffusion=True), PythonStep(MyKernel))
     assert not KernelPlan([pb.AdvectionRK4, pb.DeleteParticle], fs).stepwise  # built-ins only: one fused launch
     with pytest.raises(TypeError):
         KernelPlan([1], _fs())

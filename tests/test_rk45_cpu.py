@@ -56,6 +56,6 @@ def test_rk45_plan_checks():
         plan = KernelPlan([pb.AdvectionRK45, pb.DeleteParticle], fs, P)
     assert fs.context["RK45_min_dt"] == 1 and fs.context["RK45_max_dt"] == 86400
     assert fs.context["RK45_tol"] == 10 / fs.grid.deg2m and plan.rk45 == (10 / fs.grid.deg2m, 1.0, 86400.0)
-    assert plan.delete_on_error and not plan.stepwise
+    assert plan.kind == "rk45" and plan.delete_on_error and not plan.stepwise
     with pytest.raises(NotImplementedError):
         KernelPlan([pb.AdvectionRK45, pb.DiffusionUniformKh], fs, P)
