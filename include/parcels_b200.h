@@ -397,6 +397,25 @@ int32_t pb_decomp_set(pb_engine* e, int32_t nranks, int32_t rank, const double* 
 int32_t pb_migrate_count(pb_engine* e, int64_t* counts /* [nranks] records to send to each rank */);
 int32_t pb_migrate_pack(pb_engine* e, void* sendbuf_dev, int64_t capacity_records);
 int32_t pb_migrate_unpack(pb_engine* e, const void* recvbuf_dev, int64_t n_in);
+/* Mode D on a CURVILINEAR grid: column slabs.  The engine keeps the whole horizontal grid uploaded with
+ * pb_grid_upload_curvilinear (lon / lat, the spherical cell projections, the spatial hash -- built exactly as on one GPU) and the
+ * node columns [xi_offset, xi_offset + X) of U, V, W (pb_field_upload with X < nx: owned cells + halo).  Every search therefore
+ * finds the single-GPU cell (yi, i) with a GLOBAL column i; rank r owns the cells with col_edges[r] <= i < col_edges[r+1]
+ * (col_edges[0] = 0, col_edges[nranks] = nx - 1).  At the top of every iteration a lane runs the search of its first evaluation
+ * (same hint, same rule) and that evaluation reuses it; a lane whose cell is another rank's stops with its ei untouched
+ * (pb_report.n_migrate), one whose search finds no cell stays and raises the single-GPU error.  A stage position whose cell
+ * needs a node column outside the slab is a halo violation (state 99).  The in-kernel delivery routes by the found column;
+ * the collective transport classifies with pb_migrate_classify_columns instead of pb_migrate_count: the same search, no_hint =
+ * the hint rule of the next launch's first iteration (with resumable state resident: of the lanes whose iteration count is 0).
+ * pb_advect (fixed-step schemes, CGrid_Velocity or XLinear_Velocity) and pb_advect_rk45_resident_async (CGrid_Velocity) run on
+ * such an engine; pb_sample_velocity and pb_sample_scalar refuse it (PB_ERR_STATE: the sampling kernels index the fields by
+ * global column).  Grids whose faces overlap (duplicated wrap columns, a north fold) are not supported. */
+int32_t pb_decomp_set_columns(pb_engine* e, int32_t nranks, int32_t rank, const int64_t* col_edges, int64_t xi_offset,
+                              int32_t left_is_global, int32_t right_is_global);
+int32_t pb_migrate_classify_columns(pb_engine* e, int32_t no_hint, int64_t* counts /* [nranks] */);
+/* Device bytes the engine holds for its grid (coordinates, time axis, cell tables, cell projections, spatial hash) and for its
+ * fields (every field slot, the node-interleaved copy). */
+int32_t pb_memory_bytes(pb_engine* e, int64_t* grid_bytes, int64_t* field_bytes);
 /* AdvectionRK45 (pb_advect_rk45_resident_async) and AdvectionDiffusionM1 / EM (pb_advect_diffusion) under mode D: a lane stopped
  * mid-call continues on its new owner with its dt, next_dt and iteration count (M1 / EM: the count keys the Wiener increments,
  * so the decomposed run draws the single-GPU run's increments).  pb_particles_upload_resume makes them resident columns (after

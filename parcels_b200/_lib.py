@@ -157,6 +157,9 @@ SYMBOLS = {
     "pb_sample_scalar": (C.c_int32, [_P, C.c_int32, C.c_int32, C.c_int64, _P, _P, _P, _P, C.c_int32, _P, _P, _P, _P, _P]),
     "pb_decomp_set": (C.c_int32, [_P, C.c_int32, C.c_int32, _P, C.c_int64, C.c_int32, C.c_int32]),
     "pb_migrate_count": (C.c_int32, [_P, _P]),
+    "pb_decomp_set_columns": (C.c_int32, [_P, C.c_int32, C.c_int32, _P, C.c_int64, C.c_int32, C.c_int32]),
+    "pb_migrate_classify_columns": (C.c_int32, [_P, C.c_int32, _P]),
+    "pb_memory_bytes": (C.c_int32, [_P, _P, _P]),
     "pb_migrate_pack": (C.c_int32, [_P, _P, C.c_int64]),
     "pb_migrate_unpack": (C.c_int32, [_P, _P, C.c_int64]),
     "pb_migrate_p2p_init": (C.c_int32, [_P, C.c_int64, _P, _P]),

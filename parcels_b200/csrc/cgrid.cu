@@ -38,6 +38,11 @@ static cudaError_t launch_policy(const AdvectParams& p, cudaStream_t s) {
 
 template <class A, class D>
 static cudaError_t launch_ad(const AdvectParams& p, int nc, cudaStream_t s) {
+    if (p.g.curvilinear && p.g.decomposed) {  // column slabs (mode D)
+        if (p.g.spherical)
+            return nc == 3 ? launch_policy<CurvPolicy<A, D, 3, true, CURV_COLUMNS>>(p, s) : launch_policy<CurvPolicy<A, D, 2, true, CURV_COLUMNS>>(p, s);
+        return nc == 3 ? launch_policy<CurvPolicy<A, D, 3, false, CURV_COLUMNS>>(p, s) : launch_policy<CurvPolicy<A, D, 2, false, CURV_COLUMNS>>(p, s);
+    }
     if (p.g.curvilinear) {
         if (p.g.spherical) return nc == 3 ? launch_policy<CurvPolicy<A, D, 3, true>>(p, s) : launch_policy<CurvPolicy<A, D, 2, true>>(p, s);
         return nc == 3 ? launch_policy<CurvPolicy<A, D, 3, false>>(p, s) : launch_policy<CurvPolicy<A, D, 2, false>>(p, s);
@@ -59,6 +64,8 @@ static cudaError_t rk45_policy(const Rk45Params& q, cudaStream_t s) {
 }
 template <class A, class D>
 static cudaError_t rk45_ad(const Rk45Params& q, cudaStream_t s) {
+    if (q.base.g.curvilinear && q.base.g.decomposed)  // column slabs (mode D)
+        return q.base.g.spherical ? rk45_policy<CurvPolicy<A, D, 2, true, CURV_COLUMNS>>(q, s) : rk45_policy<CurvPolicy<A, D, 2, false, CURV_COLUMNS>>(q, s);
     if (q.base.g.curvilinear) return q.base.g.spherical ? rk45_policy<CurvPolicy<A, D, 2, true>>(q, s) : rk45_policy<CurvPolicy<A, D, 2, false>>(q, s);
     return rk45_policy<CGridPolicy<A, D, 2>>(q, s);
 }
@@ -67,6 +74,46 @@ cudaError_t launch_rk45_cgrid(const AdvectParams& p, double* dt, double* next_dt
     Rk45Params q{p, dt, next_dt, iters, next_dt_f32, tol, min_dt, max_dt};
     if (coord_f64) return data_f64 ? rk45_ad<double, double>(q, s) : rk45_ad<double, float>(q, s);
     return data_f64 ? rk45_ad<float, double>(q, s) : rk45_ad<float, float>(q, s);
+}
+
+// Column slabs (mode D), the classify pass of the collective transport: dest[i] = the rank whose cell columns [edges[r], edges[r+1])
+// hold the cell particle i's next search finds -- the ownership test the advection kernels run at the top of an iteration, with
+// the hint rule of that iteration (iters: per-particle iteration counts of the call, NULL: every particle at its first) -- or -1
+// when the particle stays (state not Evaluate, no cell found, a cell of this rank).  counts[r]: leavers per rank, counts[nranks]:
+// stayers.
+template <class Policy>
+__global__ void classify_columns_kernel(const AdvectParams p, const int* __restrict__ iters, int no_hint, const double* __restrict__ edges,
+                                        int nranks, int rank, int* dest, unsigned long long* counts) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= p.P.n) return;
+    int d = -1;
+    if (p.P.state[i] == PB_EVALUATE) {
+        typename Policy::Ctx e;
+        Policy::init(e, p, p.P.ei[i]);
+        const int col = Policy::owner_search(p, e, no_hint && (!iters || iters[i] == 0), p.P.x[i], p.P.y[i]);
+        if (col >= 0) {
+            int r = 0;
+            while (r + 1 < nranks && (double)col >= edges[r + 1]) ++r;
+            if (r != rank) d = r;
+        }
+    }
+    dest[i] = d;
+    atomicAdd(&counts[d < 0 ? nranks : d], 1ULL);
+}
+template <class A>
+static void classify_columns_a(const AdvectParams& p, const int* iters, int no_hint, const double* edges, int nranks, int rank, int* dest,
+                               unsigned long long* counts, cudaStream_t s) {
+    const unsigned grid = (unsigned)((p.P.n + 127) / 128);
+    if (p.g.spherical)
+        classify_columns_kernel<CurvPolicy<A, float, 2, true, CURV_COLUMNS>><<<grid, 128, 0, s>>>(p, iters, no_hint, edges, nranks, rank, dest, counts);
+    else
+        classify_columns_kernel<CurvPolicy<A, float, 2, false, CURV_COLUMNS>><<<grid, 128, 0, s>>>(p, iters, no_hint, edges, nranks, rank, dest, counts);
+}
+cudaError_t launch_classify_columns(const AdvectParams& p, bool coord_f64, const int* iters, int no_hint, const double* edges, int nranks,
+                                    int rank, int* dest, unsigned long long* counts, cudaStream_t s) {
+    if (coord_f64) classify_columns_a<double>(p, iters, no_hint, edges, nranks, rank, dest, counts, s);
+    else classify_columns_a<float>(p, iters, no_hint, edges, nranks, rank, dest, counts, s);
+    return cudaGetLastError();
 }
 
 template <class Policy>

@@ -565,13 +565,24 @@ struct CGridPolicy {
 // small places (depth bcoord, hash-grid quantisation, the spherical conversion factor): they branch at
 // run time and the whole search + interpolation is instantiated ONCE per kernel.
 // ------------------------------------------------------------------------------------------------
-// VEL: 0 = CGrid_Velocity, 1 = XLinear_Velocity (an A-grid on 2-D lon / lat: the reference's XGrid.search feeds the same
+// VEL (KIND & CURV_XLINEAR): 0 = CGrid_Velocity, 1 = XLinear_Velocity (an A-grid on 2-D lon / lat: the reference's XGrid.search feeds the same
 // interpolators whatever the grid's shape, _core/xgrid.py:316-356 + interpolators/_xinterpolators.py:112-190)
 template <class A, class D>
 struct CurvACtx : CGridCtx<A, D> {
     D blk[3][16];  // VEL 1: the (t, z, y, x) corner block of U, V, W of the cached cell, [component][(t*2+z)*4 + y*2 + x]
 };
-template <class A, class D, int NC_, bool SPH, int VEL = 0>
+// column slabs (mode D): the search result of an iteration's ownership test, kept for its first evaluation
+template <class Base>
+struct ColumnsCtx : Base {
+    int pyi, pxi;
+    double pxsi, peta;
+    bool pre;  // pyi .. peta are the next evaluation's search result
+};
+// KIND: the interpolator, CURV_XLINEAR or not (CGrid_Velocity), and CURV_COLUMNS: mode D on a curvilinear grid (column slabs, the
+// grid replicated), compiled apart from the single-GPU instantiations (whose template arguments -- 0 and CURV_XLINEAR -- it leaves
+// as they were)
+constexpr int CURV_XLINEAR = 1, CURV_COLUMNS = 2;
+template <class A, class D, int NC_, bool SPH, int KIND = 0>
 struct CurvPolicy {
     static constexpr int NC = NC_;
     static constexpr bool RUNTIME_DTYPE = true;
@@ -579,9 +590,15 @@ struct CurvPolicy {
     static constexpr bool F32_STAGES = false;
     static constexpr bool BATCH_LEN_T = std::is_same<A, float>::value;
     static constexpr bool BATCH_LEN_Z = false;
-    using Ctx = typename std::conditional<VEL == 1, CurvACtx<A, D>, CGridCtx<A, D>>::type;
+    static constexpr int VEL = KIND & CURV_XLINEAR;  // 0: CGrid_Velocity, 1: XLinear_Velocity
+    static constexpr bool COLUMNS = (KIND & CURV_COLUMNS) != 0;
+    using Base = typename std::conditional<VEL == 1, CurvACtx<A, D>, CGridCtx<A, D>>::type;
+    using Ctx = typename std::conditional<COLUMNS, ColumnsCtx<Base>, Base>::type;
 
-    __device__ static __forceinline__ void init(Ctx& e, const AdvectParams& p, int ei) { CGridPolicy<A, D, NC_>::init(e, p, ei); }
+    __device__ static __forceinline__ void init(Ctx& e, const AdvectParams& p, int ei) {
+        CGridPolicy<A, D, NC_>::init(e, p, ei);
+        if constexpr (COLUMNS) e.pre = false;
+    }
     __device__ static __forceinline__ void finish(Ctx&, const AdvectParams&) {}
 
     // XLinear_Velocity behind the curvilinear search: T-lerp, Z-lerp, bilinear in NumPy's dtypes (xsi, eta are float64 -- the
@@ -638,6 +655,7 @@ struct CurvPolicy {
             if (!(0 <= t && t <= g.time_len)) {
                 e.state = PB_ERROR_OUTSIDE_TIME_INTERVAL;
                 e.out_of_time = true;
+                if constexpr (COLUMNS) e.pre = false;  // (this evaluation does not search)
                 return;
             }
             tau = axis_search<double, double>(g.time, g.nt, t, e.ct);
@@ -673,6 +691,215 @@ struct CurvPolicy {
         }
         double xsi = -1.0, eta = -1.0;
         int yi, xi;
+        if constexpr (COLUMNS) {
+            if (e.pre) {  // the iteration's ownership test searched this position already (stage 1)
+                e.pre = false;
+                yi = e.pyi; xi = e.pxi; xsi = e.pxsi; eta = e.peta;
+            } else {
+                search(p, e, no_hint, x, y, xy_f32, q, yi, xi, xsi, eta);
+            }
+        } else {
+            // (a copy of this search is CurvPolicy::search below, used by the column-slab instantiations: keep both in step)
+            // `if np.any(xi)` (index_search.py:269): a batch whose hinted xi are ALL zero skips the hint test.  The host knows that for
+            // the first evaluation of a call (no_hint); a set of ONE particle knows it by itself at every evaluation.
+            const bool lone_zero = p.lone_particle && e.xi == 0;
+            const bool hint_ok = !no_hint && !lone_zero && e.yi >= 0 && e.xi >= 0 && e.yi < g.ny - 1 && e.xi < g.nx - 1;
+            bool found = false;
+            if (hint_ok) found = point_in_cell(g, e, e.yi, e.xi, q, xsi, eta);
+            if (found) {
+                yi = e.yi; xi = e.xi;
+            } else {
+                // The reference goes straight to the spatial hash.  Most misses are a move into an adjacent cell:
+                // test the 8 neighbours first and accept a hit only when (a) the point is SAFELY interior -- then
+                // that cell is the only one containing it -- and (b) the hash table lists that face under the
+                // point's hash cell (a face whose corner bounding box misses the point is invisible to the
+                // reference's query).  Then the hash's "first containing candidate" is this very cell with these
+                // very coordinates, float32-rounded like spatialhash.py:511.  Anything else -- edge-grazing
+                // points, jumps, no valid hint -- takes the exact hash path.
+                unsigned int qx, qy, qz;
+                if (xy_f32) hash_coords<A, float, float>(g, (float)y, (float)x, qx, qy, qz);
+                else if (SPH) hash_coords_xyz<A>(g, q.qu_x, q.qu_y, q.qu_z, qx, qy, qz);  // no second set of sin/cos
+                else hash_coords<A, double, double>(g, y, x, qx, qy, qz);
+                bool nb = false;
+                if (hint_ok && isfinite(x) && isfinite(y)) {
+                    const int hj = e.yi, hi = e.xi;
+                    // the failed hint test says which way the point left the hinted cell: that neighbour is tested first
+                    // (k = -1), the other seven only if it is not the one (non-overlapping cells: at most one can pass)
+                    const int gdj = eta > 1 ? 1 : (eta < 0 ? -1 : 0);
+                    const int gdi = xsi > 1 ? 1 : (xsi < 0 ? -1 : 0);
+    #pragma unroll 1
+                    for (int k = -1; k < 8 && !nb; ++k) {
+                        int dj, di;
+                        if (k < 0) {
+                            dj = gdj; di = gdi;
+                            if ((dj | di) == 0) continue;
+                        } else {
+                            dj = (k < 3) ? -1 : ((k < 5) ? 0 : 1);
+                            di = (k == 0 || k == 3 || k == 5) ? -1 : ((k == 1 || k == 6) ? 0 : 1);
+                            if (dj == gdj && di == gdi) continue;
+                        }
+                        const int j = hj + dj, i = hi + di;
+                        if (j < 0 || i < 0 || j >= g.ny - 1 || i >= g.nx - 1) continue;
+                        double cs, ce;
+                        if (point_in_cell(g, e, j, i, q, cs, ce) && cs > 1e-6 && cs < 1 - 1e-6 && ce > 1e-6 && ce < 1 - 1e-6 &&
+                            face_listed(g, j, i, qx, qy, qz)) {
+                            nb = true;
+                            yi = j; xi = i;
+                            xsi = (double)(float)cs;
+                            eta = (double)(float)ce;
+                        }
+                    }
+                }
+                if (!nb) {
+                    // (inline on purpose: out of line -- 0.03 queries per warp-step, ~350 instructions -- the call spills the caller's live
+                    //  registers)
+                    hash_query(g, e, q, xy_f32 ? isfinite((float)x) && isfinite((float)y) : isfinite(x) && isfinite(y), qx, qy, qz, yi, xi, xsi, eta);
+                }
+            }
+        }
+        e.yi = yi; e.xi = xi;
+        long long r = (long long)yi * g.xdim + (long long)xi;
+        if (g.nz > 0) r += (long long)zi * (g.ydim * g.xdim);
+        e.ei = (int)r;
+        int s = e.state;
+        if (zi == -1) s = max(s, (int)PB_ERROR_OUT_OF_BOUNDS);
+        if (xi == -3 || yi == -3) s = max(s, (int)PB_ERROR_GRID_SEARCHING);
+        if (zi == -2) s = max(s, (int)PB_ERROR_THROUGH_SURFACE);
+        e.state = s;
+        if (xi < 0 || yi < 0 || zi < 0) return;
+        // column slabs: the grid is global, the fields hold node columns [xi_offset, xi_offset + X).  The cell's node columns xi and
+        // xi + 1 (which include the C-grid face column xi + off_x) must be among them, else the halo is too small for this dt:
+        // state 99, no value
+        int fxi = xi;
+        if constexpr (COLUMNS) {
+            fxi = xi - g.xi_offset;
+            if (fxi < 0 || fxi + 1 > f.X - 1) {
+                e.state = max(e.state, 99);
+                return;
+            }
+        }
+
+        if constexpr (VEL == 1) {  // -- XLinear_Velocity (_xinterpolators.py:112-190) on the searched cell
+            const bool two_t = g.nt > 0 && (e.len_t < 0 ? (tau > 0) : (e.len_t != 0));
+            const bool two_z = g.nz > 0 && (e.len_z < 0 ? !(zeta <= 0) : (e.len_z != 0));
+            double q[3] = {0.0, 0.0, 0.0};
+            xlinear_rt(f, e, ti, tau, zi, zeta, zeta_f32, yi, eta, fxi, xsi, two_t, two_z, q);
+            if (SPH) {  // u /= deg2m * cos(deg2rad(y)) in the dtype of the sampled y; v /= deg2m  (:182-184)
+                const double conv = xy_f32 ? (double)((float)g.deg2m * cosf_ool(deg2rad_np((float)y))) : g.deg2m * cos_lat;
+                q[0] = q[0] / conv;
+                q[1] = q[1] / g.deg2m;
+            }
+            u = Val{q[0], false}; v = Val{q[1], false}; w = Val{NC_ == 3 ? q[2] : 0.0, false};
+            if (u.v != u.v || v.v != v.v || w.v != w.v) e.state = max(e.state, (int)PB_ERROR_INTERPOLATION);
+            return;
+        }
+        // -- CGrid_Velocity (_xinterpolators.py:193-332)
+        load_corners(g, e, yi, xi);
+        const bool two_t = e.len_t < 0 ? (tau > 0) : (e.len_t != 0);  // lenT: the batch's decision when known
+        A px[4], py[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) py[k] = e.clat[k];
+        if (SPH) {  // corner longitudes unwrapped relative to corner 0 (:230-233): a property of the cell, redone on a cell change only
+            if (e.uyi != yi || e.uxi != xi) {
+                e.uyi = yi; e.uxi = xi;
+#pragma unroll
+                for (int k = 0; k < 4; ++k) e.ulon[k] = mod_np((A)(e.clon[k] + (A)180.0), (A)360.0) - (A)180.0;
+#pragma unroll
+                for (int k = 1; k < 4; ++k) if (e.ulon[k] - e.ulon[0] > (A)180) e.ulon[k] = e.ulon[k] - (A)360;
+#pragma unroll
+                for (int k = 1; k < 4; ++k) if (-e.ulon[k] + e.ulon[0] > (A)180) e.ulon[k] = e.ulon[k] + (A)360;
+            }
+#pragma unroll
+            for (int k = 0; k < 4; ++k) px[k] = e.ulon[k];
+        } else {
+#pragma unroll
+            for (int k = 0; k < 4; ++k) px[k] = e.clon[k];
+        }
+        CGridPolicy<A, D, NC_>::load_faces(g, f, e, ti, zi, yi, fxi);
+        // spherical conversion factor in the dtype of the sampled y
+        double conv = 1.0;
+        if (SPH) conv = xy_f32 ? (double)((float)g.deg2m * cosf_ool(deg2rad_np((float)y))) : g.deg2m * cos_lat;
+        Val wdummy;
+        if constexpr (SPH || std::is_same<A, double>::value) {
+            // every operand the face values meet is float64 (edge lengths are float64: float64 bcoords on a
+            // spherical mesh / float64 corner coordinates), so they convert exactly: ONE float64 code path
+            double c[6];
+            if (two_t) {
+                const double omt = 1 - tau;
+                c[0] = e.fu[0] * omt + e.fu[2] * tau; c[1] = e.fu[1] * omt + e.fu[3] * tau;
+                c[2] = e.fv[0] * omt + e.fv[2] * tau; c[3] = e.fv[1] * omt + e.fv[3] * tau;
+            } else {
+                c[0] = (double)e.fu[0]; c[1] = (double)e.fu[1]; c[2] = (double)e.fv[0]; c[3] = (double)e.fv[1];
+            }
+            cgrid_finish<SPH, double, A, double, double, double, double, 2>(g, px, py, c[0], c[1], c[2], c[3], 0.0, 0.0, 0.0, eta, xsi,
+                                                                            conv, u, v, wdummy);
+        } else {  // flat mesh with float32 corner coordinates: edge lengths are float32, the face dtype matters
+            if (two_t) {
+                const double omt = 1 - tau;
+                cgrid_finish<SPH, double, A, double, double, double, double, 2>(g, px, py, e.fu[0] * omt + e.fu[2] * tau,
+                                                                                e.fu[1] * omt + e.fu[3] * tau, e.fv[0] * omt + e.fv[2] * tau,
+                                                                                e.fv[1] * omt + e.fv[3] * tau, 0.0, 0.0, 0.0, eta, xsi, conv, u,
+                                                                                v, wdummy);
+            } else {
+                cgrid_finish<SPH, D, A, double, double, double, double, 2>(g, px, py, e.fu[0], e.fu[1], e.fv[0], e.fv[1], (D)0, (D)0, 0.0, eta,
+                                                                           xsi, conv, u, v, wdummy);
+            }
+        }
+        if (NC_ == 3) {  // W: linear in zeta between the two Z faces (:316-330); dtype as NumPy would promote
+            const bool tl = two_t;
+            if (!tl && std::is_same<D, float>::value && zeta_f32) {
+                const float zf = (float)zeta;
+                const float wr = (float)e.fw[0] * (1 - zf) + (float)e.fw[1] * zf;
+                w = Val{(double)wr, true};
+            } else {
+                const double omt = 1 - tau;
+                const double w0 = tl ? e.fw[0] * omt + e.fw[2] * tau : (double)e.fw[0];
+                const double w1 = tl ? e.fw[1] * omt + e.fw[3] * tau : (double)e.fw[1];
+                const double omz = zeta_f32 ? (double)(1 - (float)zeta) : 1 - zeta;
+                w = Val{w0 * omz + w1 * zeta, false};
+            }
+        } else {
+            w = Val{0.0, u.f32};
+        }
+        if (u.v != u.v || v.v != v.v || w.v != w.v) e.state = max(e.state, (int)PB_ERROR_INTERPOLATION);
+    }
+
+    // the unit-sphere query of a position (spherical meshes; cos_lat: cos(deg2rad(y)) in float64)
+    __device__ static __forceinline__ Query query(double x, double y, double& cos_lat) {
+        Query q;
+        q.x = x; q.y = y;
+        q.qu_x = q.qu_y = q.qu_z = 0.0;
+        if (SPH) {
+            const double la = deg2rad_np(y), lo = deg2rad_np(x);
+            const double cl = cos_np(la);
+            cos_lat = cl;
+            double sl, cl2;
+            sincos_lon(lo, sl, cl2);
+            q.qu_x = cl2 * cl; q.qu_y = sl * cl; q.qu_z = sin_lat(la);
+        }
+        return q;
+    }
+
+    // Column slabs (mode D on a curvilinear grid): the ownership test of an iteration -- the search of its first evaluation run
+    // ahead (same hint, same rule), kept for that evaluation to reuse.  Returns the GLOBAL cell column found, -1 when none.
+    __device__ static __forceinline__ int owner_search(const AdvectParams& p, Ctx& e, bool no_hint, float x, float y) {
+        if constexpr (COLUMNS) {
+            double cos_lat = 1.0;
+            const Query q = query((double)x, (double)y, cos_lat);
+            search(p, e, no_hint, (double)x, (double)y, true, q, e.pyi, e.pxi, e.pxsi, e.peta);
+            e.pre = true;
+            return e.pxi >= 0 && e.pyi >= 0 ? e.pxi : -1;
+        }
+        return -1;
+    }
+
+    // eval_rt's search (hint, neighbours, hash) for the column-slab instantiations: the single-GPU ones keep it written out in
+    // eval_rt, where their code is the measured one (the same SASS as before column slabs existed).  TWO COPIES: a change to the
+    // search goes into both, this one and the `else` branch of eval_rt's search; likewise query() and eval_rt's query.
+    __device__ static __forceinline__ void search(const AdvectParams& p, Ctx& e, bool no_hint, double x, double y, bool xy_f32,
+                                                  const Query& q, int& yi, int& xi, double& xsi, double& eta) {
+        const GridDev& g = p.g;
+        xsi = -1.0; eta = -1.0;
         // `if np.any(xi)` (index_search.py:269): a batch whose hinted xi are ALL zero skips the hint test.  The host knows that for
         // the first evaluation of a call (no_hint); a set of ONE particle knows it by itself at every evaluation.
         const bool lone_zero = p.lone_particle && e.xi == 0;
@@ -729,100 +956,6 @@ struct CurvPolicy {
                 hash_query(g, e, q, xy_f32 ? isfinite((float)x) && isfinite((float)y) : isfinite(x) && isfinite(y), qx, qy, qz, yi, xi, xsi, eta);
             }
         }
-        e.yi = yi; e.xi = xi;
-        long long r = (long long)yi * g.xdim + (long long)xi;
-        if (g.nz > 0) r += (long long)zi * (g.ydim * g.xdim);
-        e.ei = (int)r;
-        int s = e.state;
-        if (zi == -1) s = max(s, (int)PB_ERROR_OUT_OF_BOUNDS);
-        if (xi == -3 || yi == -3) s = max(s, (int)PB_ERROR_GRID_SEARCHING);
-        if (zi == -2) s = max(s, (int)PB_ERROR_THROUGH_SURFACE);
-        e.state = s;
-        if (xi < 0 || yi < 0 || zi < 0) return;
-
-        if constexpr (VEL == 1) {  // -- XLinear_Velocity (_xinterpolators.py:112-190) on the searched cell
-            const bool two_t = g.nt > 0 && (e.len_t < 0 ? (tau > 0) : (e.len_t != 0));
-            const bool two_z = g.nz > 0 && (e.len_z < 0 ? !(zeta <= 0) : (e.len_z != 0));
-            double q[3] = {0.0, 0.0, 0.0};
-            xlinear_rt(f, e, ti, tau, zi, zeta, zeta_f32, yi, eta, xi, xsi, two_t, two_z, q);
-            if (SPH) {  // u /= deg2m * cos(deg2rad(y)) in the dtype of the sampled y; v /= deg2m  (:182-184)
-                const double conv = xy_f32 ? (double)((float)g.deg2m * cosf_ool(deg2rad_np((float)y))) : g.deg2m * cos_lat;
-                q[0] = q[0] / conv;
-                q[1] = q[1] / g.deg2m;
-            }
-            u = Val{q[0], false}; v = Val{q[1], false}; w = Val{NC_ == 3 ? q[2] : 0.0, false};
-            if (u.v != u.v || v.v != v.v || w.v != w.v) e.state = max(e.state, (int)PB_ERROR_INTERPOLATION);
-            return;
-        }
-        // -- CGrid_Velocity (_xinterpolators.py:193-332)
-        load_corners(g, e, yi, xi);
-        const bool two_t = e.len_t < 0 ? (tau > 0) : (e.len_t != 0);  // lenT: the batch's decision when known
-        A px[4], py[4];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) py[k] = e.clat[k];
-        if (SPH) {  // corner longitudes unwrapped relative to corner 0 (:230-233): a property of the cell, redone on a cell change only
-            if (e.uyi != yi || e.uxi != xi) {
-                e.uyi = yi; e.uxi = xi;
-#pragma unroll
-                for (int k = 0; k < 4; ++k) e.ulon[k] = mod_np((A)(e.clon[k] + (A)180.0), (A)360.0) - (A)180.0;
-#pragma unroll
-                for (int k = 1; k < 4; ++k) if (e.ulon[k] - e.ulon[0] > (A)180) e.ulon[k] = e.ulon[k] - (A)360;
-#pragma unroll
-                for (int k = 1; k < 4; ++k) if (-e.ulon[k] + e.ulon[0] > (A)180) e.ulon[k] = e.ulon[k] + (A)360;
-            }
-#pragma unroll
-            for (int k = 0; k < 4; ++k) px[k] = e.ulon[k];
-        } else {
-#pragma unroll
-            for (int k = 0; k < 4; ++k) px[k] = e.clon[k];
-        }
-        CGridPolicy<A, D, NC_>::load_faces(g, f, e, ti, zi, yi, xi);
-        // spherical conversion factor in the dtype of the sampled y
-        double conv = 1.0;
-        if (SPH) conv = xy_f32 ? (double)((float)g.deg2m * cosf_ool(deg2rad_np((float)y))) : g.deg2m * cos_lat;
-        Val wdummy;
-        if constexpr (SPH || std::is_same<A, double>::value) {
-            // every operand the face values meet is float64 (edge lengths are float64: float64 bcoords on a
-            // spherical mesh / float64 corner coordinates), so they convert exactly: ONE float64 code path
-            double c[6];
-            if (two_t) {
-                const double omt = 1 - tau;
-                c[0] = e.fu[0] * omt + e.fu[2] * tau; c[1] = e.fu[1] * omt + e.fu[3] * tau;
-                c[2] = e.fv[0] * omt + e.fv[2] * tau; c[3] = e.fv[1] * omt + e.fv[3] * tau;
-            } else {
-                c[0] = (double)e.fu[0]; c[1] = (double)e.fu[1]; c[2] = (double)e.fv[0]; c[3] = (double)e.fv[1];
-            }
-            cgrid_finish<SPH, double, A, double, double, double, double, 2>(g, px, py, c[0], c[1], c[2], c[3], 0.0, 0.0, 0.0, eta, xsi,
-                                                                            conv, u, v, wdummy);
-        } else {  // flat mesh with float32 corner coordinates: edge lengths are float32, the face dtype matters
-            if (two_t) {
-                const double omt = 1 - tau;
-                cgrid_finish<SPH, double, A, double, double, double, double, 2>(g, px, py, e.fu[0] * omt + e.fu[2] * tau,
-                                                                                e.fu[1] * omt + e.fu[3] * tau, e.fv[0] * omt + e.fv[2] * tau,
-                                                                                e.fv[1] * omt + e.fv[3] * tau, 0.0, 0.0, 0.0, eta, xsi, conv, u,
-                                                                                v, wdummy);
-            } else {
-                cgrid_finish<SPH, D, A, double, double, double, double, 2>(g, px, py, e.fu[0], e.fu[1], e.fv[0], e.fv[1], (D)0, (D)0, 0.0, eta,
-                                                                           xsi, conv, u, v, wdummy);
-            }
-        }
-        if (NC_ == 3) {  // W: linear in zeta between the two Z faces (:316-330); dtype as NumPy would promote
-            const bool tl = two_t;
-            if (!tl && std::is_same<D, float>::value && zeta_f32) {
-                const float zf = (float)zeta;
-                const float wr = (float)e.fw[0] * (1 - zf) + (float)e.fw[1] * zf;
-                w = Val{(double)wr, true};
-            } else {
-                const double omt = 1 - tau;
-                const double w0 = tl ? e.fw[0] * omt + e.fw[2] * tau : (double)e.fw[0];
-                const double w1 = tl ? e.fw[1] * omt + e.fw[3] * tau : (double)e.fw[1];
-                const double omz = zeta_f32 ? (double)(1 - (float)zeta) : 1 - zeta;
-                w = Val{w0 * omz + w1 * zeta, false};
-            }
-        } else {
-            w = Val{0.0, u.f32};
-        }
-        if (u.v != u.v || v.v != v.v || w.v != w.v) e.state = max(e.state, (int)PB_ERROR_INTERPOLATION);
     }
 };
 

@@ -14,6 +14,11 @@ static cudaError_t launch_policy(const AdvectParams& p, cudaStream_t s) {
 }
 template <class A, class D>
 static cudaError_t launch_ad(const AdvectParams& p, int nc, cudaStream_t s) {
+    if (p.g.decomposed) {  // column slabs (mode D)
+        if (p.g.spherical)
+            return nc == 3 ? launch_policy<CurvPolicy<A, D, 3, true, CURV_XLINEAR | CURV_COLUMNS>>(p, s) : launch_policy<CurvPolicy<A, D, 2, true, CURV_XLINEAR | CURV_COLUMNS>>(p, s);
+        return nc == 3 ? launch_policy<CurvPolicy<A, D, 3, false, CURV_XLINEAR | CURV_COLUMNS>>(p, s) : launch_policy<CurvPolicy<A, D, 2, false, CURV_XLINEAR | CURV_COLUMNS>>(p, s);
+    }
     if (p.g.spherical) return nc == 3 ? launch_policy<CurvPolicy<A, D, 3, true, 1>>(p, s) : launch_policy<CurvPolicy<A, D, 2, true, 1>>(p, s);
     return nc == 3 ? launch_policy<CurvPolicy<A, D, 3, false, 1>>(p, s) : launch_policy<CurvPolicy<A, D, 2, false, 1>>(p, s);
 }

@@ -988,6 +988,13 @@ static int32_t field_slot_desc(pb_engine* e, int32_t slot, FieldDev& f) {
 }
 
 
+// Column slabs (pb_decomp_set_columns): the grid is global, the fields hold a column slab.  Only the column-slab instantiations of
+// the advection kernels (CurvPolicy with CURV_COLUMNS) shift the found global column into the slab and test the halo; the sampling
+// kernels would read the slab at global columns, past its end, so sampling is refused on such an engine.
+static bool on_columns(const pb_engine* e) { return e->g.curvilinear && e->g.decomposed; }
+static const char* const COLUMNS_NO_SAMPLING =
+    "field sampling is not available on a column slab of a curvilinear grid (mode D): sample the undecomposed FieldSet";
+
 // validation shared by pb_advect and pb_sample_velocity; nc = 2 (UV) or 3 (UVW)
 static int32_t check_fields(pb_engine* e, int nc) {
     if (!e->have_grid) return fail(PB_ERR_STATE, "grid not uploaded (pb_grid_upload_*)");
@@ -999,7 +1006,9 @@ static int32_t check_fields(pb_engine* e, int nc) {
             if (e->fshape[c][d] != e->fshape[0][d]) return fail(PB_ERR_INVALID, "U, V, W must share one shape");
     }
     const long long T = e->fshape[0][0], Z = e->fshape[0][1], Y = e->fshape[0][2], X = e->fshape[0][3];
-    if ((X > 1 && X != e->g.nx) || (Y > 1 && Y != e->g.ny) || (Z > 1 && e->g.nz > 0 && Z != e->g.nz) ||
+    // column slabs (pb_decomp_set_columns): the fields hold node columns [xi_offset, xi_offset + X) of the global grid
+    const bool columns = on_columns(e);
+    if ((X > 1 && X != e->g.nx && !(columns && X >= 2 && e->g.xi_offset + X <= e->g.nx)) || (Y > 1 && Y != e->g.ny) || (Z > 1 && e->g.nz > 0 && Z != e->g.nz) ||
         (T > 1 && e->g.nt > 0 && T != e->g.nt))
         return fail(PB_ERR_INVALID, "field shape (%lld,%lld,%lld,%lld) does not match grid nodes (nt=%d nz=%d ny=%d nx=%d)", T, Z, Y, X,
                     e->g.nt, e->g.nz, e->g.ny, e->g.nx);
@@ -1029,6 +1038,7 @@ int32_t pb_sample_velocity(pb_engine* e, int64_t n, const double* t, const doubl
     if (!e) return fail(PB_ERR_INVALID, "engine is NULL");
     if (n < 0 || (n && (!t || !z || !y || !x || !u || !v || !w || !ei_out || !state_out))) return fail(PB_ERR_INVALID, "NULL argument");
     const int nc = three_d ? 3 : 2;
+    if (on_columns(e)) return fail(PB_ERR_STATE, "%s", COLUMNS_NO_SAMPLING);
     int32_t rc = check_fields(e, nc);
     if (rc) return rc;
     if (n == 0) return PB_OK;
@@ -1075,6 +1085,7 @@ int32_t pb_sample_scalar(pb_engine* e, int32_t slot, int32_t method, int64_t n, 
     if (slot < 0 || slot >= PB_MAX_FIELDS || !e->fptr[slot]) return fail(PB_ERR_STATE, "no field in slot %d", slot);
     if (method < PB_SCALAR_XLINEAR || method > PB_SCALAR_XLINEAR_INVDIST_LAND) return fail(PB_ERR_INVALID, "unknown scalar interpolation %d", method);
     if (!e->have_grid) return fail(PB_ERR_STATE, "grid not uploaded (pb_grid_upload_*)");
+    if (on_columns(e)) return fail(PB_ERR_STATE, "%s", COLUMNS_NO_SAMPLING);
     if (e->g.curvilinear && method == PB_SCALAR_XLINEAR_INVDIST_LAND)
         return fail(PB_ERR_INVALID, "on curvilinear grids scalar sampling is implemented for XLinear, CGrid_Tracer and XNearest");
     if (e->ring && slot < 3) return fail(PB_ERR_INVALID, "U, V, W are time-windowed: sample them through pb_sample_velocity");
@@ -1165,6 +1176,10 @@ static void fill_advect_params(pb_engine* e, const Args* a, AdvectParams& p) {
 }
 }
 
+// AdvectParams::lone_particle: the resident set is the whole set and holds one particle.  (Under mode D a rank holds a shard:
+// its count says nothing about the whole set, and a shard of one particle is no batch of one.)
+static int lone_particle(const pb_engine* e) { return e->n == 1 && !e->g.decomposed; }
+
 // in-kernel migration (connected over peer memory, mode D): where the kernels deliver a leaving particle
 static int32_t fill_mig(pb_engine* e, AdvectParams& p) {
     if (e->mig_on && e->g.decomposed) {
@@ -1222,7 +1237,7 @@ int32_t pb_advect_async(pb_engine* e, const pb_advect_args* a) {
     if (rc) return rc;
     if (a->diffusion && !e->have_pid) return fail(PB_ERR_STATE, "diffusion needs particle_id (RNG counter)");
     CK(cudaSetDevice(e->device));
-    p.lone_particle = e->n == 1;
+    p.lone_particle = lone_particle(e);
     if ((rc = begin_launch(e))) return rc;
     if (e->n > 0) {
         cudaError_t ce = launch_advect_kernel(e, p, nc, e->stream);
@@ -1438,14 +1453,15 @@ int32_t pb_advect_rk45_resident_async(pb_engine* e, const pb_rk45_args* a) {
     if (rc) return rc;
     const bool cgrid = e->interp == PB_INTERP_CGRID_VELOCITY;
     const bool slip = agrid_alt_mode(e->interp) == 1;
-    if (!(cgrid || e->interp == PB_INTERP_XLINEAR_VELOCITY || slip) || e->g.curvilinear)
+    if (!(cgrid || ((e->interp == PB_INTERP_XLINEAR_VELOCITY || slip) && !e->g.curvilinear)))
         return fail(PB_ERR_INVALID, "pb_advect_rk45_resident runs on rectilinear grids with XLinear_Velocity, XFreeslip, XPartialslip "
-                                    "or CGrid_Velocity");
+                                    "or on rectilinear and curvilinear grids with CGrid_Velocity");
     CK(cudaSetDevice(e->device));
     AdvectParams p{};
     fill_advect_params(e, a, p);
     p.scheme = PB_ADVECTION_RK45;
-    p.lone_particle = e->n == 1;
+    p.hint_all_zero = a->hint_all_zero;
+    p.lone_particle = lone_particle(e);
     if ((rc = fill_mig(e, p))) return rc;
     if ((rc = begin_launch(e))) return rc;
     if (e->n > 0) {
@@ -1633,6 +1649,81 @@ int32_t pb_decomp_set(pb_engine* e, int32_t nranks, int32_t rank, const double* 
     e->g.own_lo = rank == 0 ? -HUGE_VAL : bounds[rank];
     e->g.own_hi = rank == nranks - 1 ? HUGE_VAL : bounds[rank + 1];
     e->send_counts.assign(nranks, 0);
+    return PB_OK;
+}
+
+// Column slabs of a curvilinear grid: the engine holds the WHOLE horizontal grid (lon / lat, cell projections, spatial hash) and
+// the node columns [xi_offset, xi_offset + X) of the fields; rank r owns the cells whose global column i has
+// col_edges[r] <= i < col_edges[r + 1].  The edges are kept as doubles in the slab-bounds buffer: the kernels' routing loop
+// compares the found column with them as the rectilinear one compares x with longitudes.
+int32_t pb_decomp_set_columns(pb_engine* e, int32_t nranks, int32_t rank, const int64_t* col_edges, int64_t xi_offset,
+                              int32_t left_is_global, int32_t right_is_global) {
+    if (!e || !col_edges) return fail(PB_ERR_INVALID, "NULL argument");
+    if (nranks < 1 || rank < 0 || rank >= nranks) return fail(PB_ERR_INVALID, "bad rank %d of %d", rank, nranks);
+    if (!e->have_grid || !e->g.curvilinear) return fail(PB_ERR_STATE, "column slabs need an uploaded curvilinear grid");
+    if (col_edges[0] != 0 || col_edges[nranks] != e->g.nx - 1) return fail(PB_ERR_INVALID, "column edges must span cells 0 .. nx - 1");
+    for (int r = 0; r < nranks; ++r)
+        if (!(col_edges[r] < col_edges[r + 1])) return fail(PB_ERR_INVALID, "column edges must be strictly increasing");
+    if (xi_offset < 0 || xi_offset > col_edges[rank] || (left_is_global != 0) != (xi_offset == 0))
+        return fail(PB_ERR_INVALID, "bad column offset %lld for the cells of rank %d", (long long)xi_offset, rank);
+    std::vector<double> edges(nranks + 1);
+    for (int r = 0; r <= nranks; ++r) edges[r] = (double)col_edges[r];
+    CK(cudaSetDevice(e->device));
+    int32_t rc = upload(e, e->mbounds, edges.data(), edges.size() * sizeof(double));
+    if (rc) return rc;
+    CK(cudaStreamSynchronize(e->stream));
+    e->nranks = nranks; e->rank = rank;
+    e->g.decomposed = nranks > 1 ? 1 : 0;
+    e->g.xi_offset = (int)xi_offset;
+    e->g.left_global = left_is_global ? 1 : 0;
+    e->g.right_global = right_is_global ? 1 : 0;
+    e->g.own_lo = edges[rank];
+    e->g.own_hi = edges[rank + 1];
+    e->send_counts.assign(nranks, 0);
+    return PB_OK;
+}
+
+int32_t pb_migrate_classify_columns(pb_engine* e, int32_t no_hint, int64_t* counts) {
+    PB_RANGE("pb_migrate_classify_columns");
+    if (!e || !counts) return fail(PB_ERR_INVALID, "NULL argument");
+    if (!e->g.curvilinear || e->nranks < 1 || e->mbounds.bytes == 0) return fail(PB_ERR_STATE, "pb_decomp_set_columns not called");
+    if (!e->have_pid && e->n) return fail(PB_ERR_STATE, "migration needs particle_id");
+    CK(cudaSetDevice(e->device));
+    const int nr = e->nranks;
+    int32_t rc;
+    if ((rc = e->mdest.ensure(e->n ? e->n * 4 : 4))) return rc;
+    if ((rc = e->mcount.ensure((size_t)(nr + 1) * 8))) return rc;
+    CK(cudaMemsetAsync(e->mcount.p, 0, (size_t)(nr + 1) * 8, e->stream));
+    if (e->n > 0) {
+        AdvectParams p{};
+        p.g = e->g;
+        p.P = e->cur.view(e->n);
+        p.hint_all_zero = no_hint;
+        // the kernels that count their iterations across ranks (resumable state resident) skip the hint at a lane's first only
+        const int* iters = e->resume_on ? e->cur.resume().iters : nullptr;
+        cudaError_t ce = launch_classify_columns(p, e->coord_f64 != 0, iters, no_hint, (const double*)e->mbounds.p, nr, e->rank,
+                                                 (int*)e->mdest.p, (unsigned long long*)e->mcount.p, e->stream);
+        if (ce != cudaSuccess) return fail(PB_ERR_CUDA, "classify_columns_kernel launch failed: %s", cudaGetErrorString(ce));
+    }
+    std::vector<unsigned long long> h(nr + 1);
+    CK(cudaMemcpyAsync(h.data(), e->mcount.p, (size_t)(nr + 1) * 8, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    e->n_send = 0;
+    for (int r = 0; r < nr; ++r) { counts[r] = (int64_t)h[r]; e->send_counts[r] = (long long)h[r]; e->n_send += (long long)h[r]; }
+    e->n_keep = (long long)h[nr];
+    return PB_OK;
+}
+
+int32_t pb_memory_bytes(pb_engine* e, int64_t* grid_bytes, int64_t* field_bytes) {
+    if (!e || !grid_bytes || !field_bytes) return fail(PB_ERR_INVALID, "NULL argument");
+    int64_t g = 0, f = 0;
+    for (const DevBuf* b : {&e->lon, &e->lat, &e->depth, &e->time, &e->hkeys, &e->hstarts, &e->hcounts, &e->hfaces, &e->hbucket,
+                            &e->cellproj, &e->hqbox, &e->cells})
+        g += (int64_t)b->bytes;
+    for (const DevBuf& b : e->fbuf) f += (int64_t)b.bytes;
+    f += (int64_t)e->il.bytes;
+    *grid_bytes = g;
+    *field_bytes = f;
     return PB_OK;
 }
 

@@ -49,13 +49,22 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, PB_MINBLOCKS) rk45_kernel(co
         // a resumed launch of the same Kernel.execute call (time-slab streaming) continues the lane's iteration count, so the
         // first-iteration batch rules, max_iters and the finalize clamp see the iterations of the whole call
         long long it = (p.resume && !p.kernels_only) ? (long long)q.iters[i] : 0;
+        [[maybe_unused]] int mig_col = -1;  // column slabs: the column of the cell a leaving lane's search found
         for (;; ++it) {
             if (p.max_iters >= 0 && it >= p.max_iters) break;
             const double tte = sign * (p.endtime - t);
             if (!((e.state == PB_SUCCESS || e.state == PB_EVALUATE) && tte >= 0)) break;
             // mode D: not ours (any more).  Tested before the window wait: the new owner, whose window slides in lock-step with this
             // one, makes the same wait decision
-            if (p.g.decomposed && !((double)x >= p.g.own_lo && (double)x < p.g.own_hi)) {
+            if constexpr (columns_v<Policy>) {
+                // column slabs: the owner of the cell the first attempt's first search finds (that search, run here and reused)
+                const int col = Policy::owner_search(p, e, it == 0 && first_attempt && p.hint_all_zero, x, y);
+                if (col >= 0 && !((double)col >= p.g.own_lo && (double)col < p.g.own_hi)) {
+                    tally.migrate = true;
+                    mig_col = col;
+                    break;
+                }
+            } else if (p.g.decomposed && !((double)x >= p.g.own_lo && (double)x < p.g.own_hi)) {
                 tally.migrate = true;
                 break;
             }
@@ -168,7 +177,8 @@ __global__ void __launch_bounds__(PB_BLOCK_THREADS, PB_MINBLOCKS) rk45_kernel(co
         q.iters[i] = (int)it;
         if (tally.migrate && p.mig.on) {
             const MigResume rs{dt, ndt, (int)it, 0};
-            tally.migrate = mig_deliver(p, i, L, tally.state, e.ei, &rs);
+            if constexpr (columns_v<Policy>) tally.migrate = mig_deliver_column(p, i, mig_col, L, tally.state, e.ei, &rs);
+            else tally.migrate = mig_deliver(p, i, L, tally.state, e.ei, &rs);
         }
     }
     publish(tally, p.rep);

@@ -5,7 +5,9 @@ contiguously by rank.  Particles do not interact on this path, so the step loop 
 ``torch.distributed`` only assembles results / timings (NCCL on GPUs, gloo in the CPU tests).
 
 Mode D (domain decomposition, config 5): the rectilinear field is cut into X-slabs (+ halo columns), one per
-GPU; a particle is advanced by the rank that owns its longitude and MIGRATES when it leaves the slab.
+GPU; a particle is advanced by the rank that owns its longitude and MIGRATES when it leaves the slab.  A curvilinear field is cut
+into COLUMN slabs instead (``DecomposedFieldSet.from_curvilinear``): every rank holds the whole horizontal grid and its spatial hash,
+only U, V, W are cut, and a particle belongs to the rank that owns the cell column its search finds.
 Two transports:
 
 * **peer memory (default over NCCL, one box)** -- ``connect_p2p``: every rank owns an inbox in its HBM that its
@@ -108,6 +110,26 @@ def slab_plan(lon, world: int, halo_cells: int) -> list[dict]:
     return plans
 
 
+def column_slab_plan(nx_nodes: int, world: int, halo_cells: int) -> list[dict]:
+    """Cut the cell columns 0 .. nx_nodes - 2 of a curvilinear grid into ``world`` slabs.
+
+    Returns per rank: ``col_edges`` (world+1 cell-column edges, shared by all ranks: rank r owns the cells whose column i has
+    col_edges[r] <= i < col_edges[r+1]), the inclusive local node-column range [lo, hi] = owned cells +- halo, ``xi_offset`` = lo,
+    and whether each local edge is a global edge."""
+    nx = int(nx_nodes)
+    ncell = nx - 1
+    if world > ncell:
+        raise ValueError(f"cannot cut {ncell} cell columns into {world} slabs")
+    edges = np.asarray([round(r * ncell / world) for r in range(world + 1)], dtype=np.int64)
+    plans = []
+    for r in range(world):
+        lo = max(0, int(edges[r]) - halo_cells)
+        hi = min(nx - 1, int(edges[r + 1]) + halo_cells)
+        plans.append(dict(rank=r, col_edges=edges, lo=lo, hi=hi, xi_offset=lo, left_global=lo == 0, right_global=hi == nx - 1,
+                          own_cells=(int(edges[r]), int(edges[r + 1]))))  # fmt: skip
+    return plans
+
+
 def route_counts(x, bounds) -> np.ndarray:
     """Host restatement of the device classify kernel: owner rank of each x (used by the CPU tests)."""
     b = np.asarray(bounds)
@@ -142,7 +164,8 @@ class DecomposedFieldSet:
 
         if np.ndim(lon) != 1 or np.ndim(lat) != 1:
             raise NotImplementedError("domain decomposition cuts rectilinear grids (1-D lon / lat) into longitude slabs; on a "
-                                      "curvilinear grid a slab is not a range of longitudes")  # fmt: skip
+                                      "curvilinear grid a slab is not a range of longitudes: use "
+                                      "DecomposedFieldSet.from_curvilinear (column slabs)")  # fmt: skip
         self.rank, self.world, self.device = rank, world, device
         self.plan = slab_plan(lon, world, halo_cells)[rank]
         lo, hi = self.plan["lo"], self.plan["hi"]
@@ -157,30 +180,65 @@ class DecomposedFieldSet:
                                        xdim=np.asarray(lon).size - 1)  # fmt: skip  (GLOBAL cell count: ei stays global)
         self._attach()
 
-    def add_field(self, name, data, interp_method="linear", time_window=None):
-        """``FieldSet.add_field`` of a GLOBAL (T, Z, Y, X) field on the velocity grid (e.g. Kh_zonal / Kh_meridional of
-        AdvectionDiffusionM1 / EM), cut to this rank's columns -- one time level at a time when it streams (``time_window``)."""
-        sl = slice(self.plan["lo"], self.plan["hi"] + 1)
-        slab = np.ascontiguousarray(np.asarray(data)[..., sl]) if time_window is None else _SlabLevels(data, sl)
-        return self.fs.add_field(name, slab, interp_method=interp_method, time_window=time_window)
-
     def add_context(self, name, value):
         """``FieldSet.add_context`` (``dres``, ``RK45_tol``, ``RK45_min_dt``, ``RK45_max_dt``, ...)."""
         self.fs.add_context(name, value)
 
     @classmethod
+    def from_curvilinear(cls, *, lon, lat, U, V, W=None, depth=None, time=None, mesh="spherical", rank, world, halo_cells=4, device=0,
+                         time_window=None, interp_method="cgrid_velocity", padding=("low", "low", "high")):  # fmt: skip
+        """This rank's COLUMN SLAB of a curvilinear FieldSet: ``lon`` / ``lat`` are the (ny, nx) node coordinates, U, V (, W) global
+        (T, Z, Y, X) fields.  Every rank holds the whole horizontal grid -- coordinates, cell projections and the spatial hash,
+        built exactly as on one GPU, so that every search finds the single-GPU cell -- and only the node columns of its owned
+        cells +- ``halo_cells`` of the fields (``column_slab_plan``).  A particle is advanced by the rank that owns the column of
+        the cell its search finds.  ``interp_method``: "cgrid_velocity" (CGrid_Velocity, SGRID ``padding``) or "linear"
+        (XLinear_Velocity).  Grids whose faces overlap (duplicated wrap columns, a north fold) are not supported."""
+        from .fieldset import FieldSet
+
+        if np.ndim(lon) != 2 or np.ndim(lat) != 2:
+            raise ValueError("from_curvilinear takes (ny, nx) node coordinates; rectilinear grids: DecomposedFieldSet(...)")
+        plan = column_slab_plan(np.shape(lon)[1], world, halo_cells)[rank]
+        sl = slice(plan["lo"], plan["hi"] + 1)
+        if time_window is None:
+            cut = lambda a: np.ascontiguousarray(np.asarray(a)[..., sl])  # noqa: E731
+        else:
+            cut = lambda a: _SlabLevels(a, sl)  # noqa: E731
+        fs = FieldSet.from_arrays(lon=lon, lat=lat, depth=depth, time=time, U=cut(U), V=cut(V), W=None if W is None else cut(W),
+                                  mesh=mesh, time_window=time_window, interp_method=interp_method, padding=padding)  # fmt: skip
+        return cls.from_slab(fs, plan, rank=rank, world=world, device=device)
+
+    @classmethod
     def from_slab(cls, fs, plan, *, rank, world, device):
-        """Wrap a FieldSet that already holds ONLY this rank's slab (built with the GLOBAL ``xdim``), e.g. when
-        every rank generates / reads just its own columns."""
+        """Wrap a FieldSet that already holds ONLY this rank's slab, e.g. when every rank generates / reads just its own columns:
+        on a rectilinear grid a slab of lon built with the GLOBAL ``xdim`` (``plan`` from ``slab_plan``), on a curvilinear grid
+        the whole (ny, nx) lon / lat with fields of the node columns [lo, hi] (``plan`` from ``column_slab_plan``)."""
         self = cls.__new__(cls)
         self.rank, self.world, self.device, self.plan, self.fs = rank, world, device, plan, fs
         self._attach()
         return self
 
+    @property
+    def columns(self) -> bool:
+        """Column slabs of a curvilinear grid (``from_curvilinear``)."""
+        return "col_edges" in self.plan
+
+    def add_field(self, name, data, interp_method="linear", time_window=None):
+        """``FieldSet.add_field`` of a GLOBAL (T, Z, Y, X) field on the velocity grid (e.g. Kh_zonal / Kh_meridional of
+        AdvectionDiffusionM1 / EM), cut to this rank's columns -- one time level at a time when it streams (``time_window``)."""
+        if self.columns:
+            raise NotImplementedError("column slabs of a curvilinear grid hold U, V and W only")
+        sl = slice(self.plan["lo"], self.plan["hi"] + 1)
+        slab = np.ascontiguousarray(np.asarray(data)[..., sl]) if time_window is None else _SlabLevels(data, sl)
+        return self.fs.add_field(name, slab, interp_method=interp_method, time_window=time_window)
+
     def _attach(self):
         self.engine = self.fs.engine(self.device)
-        self.engine.decomp_set(self.world, self.rank, self.plan["bounds"], self.plan["xi_offset"], self.plan["left_global"],
-                               self.plan["right_global"])  # fmt: skip
+        if self.columns:
+            self.engine.decomp_set_columns(self.world, self.rank, self.plan["col_edges"], self.plan["xi_offset"], self.plan["left_global"],
+                                           self.plan["right_global"])  # fmt: skip
+        else:
+            self.engine.decomp_set(self.world, self.rank, self.plan["bounds"], self.plan["xi_offset"], self.plan["left_global"],
+                                   self.plan["right_global"])  # fmt: skip
 
 
 def _engine_memory_device(index: int):
@@ -289,7 +347,17 @@ def _carries_resume(plan) -> bool:
     return plan.kind in ("rk45", "advdiff")
 
 
-def _advect_args(eng, plan, dt, endtime, first, seed, rng_call, rounds):
+def _first_eval_hint(dfs, plan, first, slid) -> bool:
+    """Column slabs: ``hint_all_zero`` of a round's launch -- the whole set's (``plan.hint_all_zero``, one all-reduce) where a
+    launch of the single-GPU call would pass it.  AdvectionRK45 passes it to every launch (its lanes count their iterations across
+    rounds and skip the hint at their first only); the fixed-step kernel, whose count restarts in every launch, gets it where a
+    single-GPU launch starts: the call's first round and, on a time-windowed field, the first round after a slide."""
+    if not dfs.columns or not plan.hint_all_zero:
+        return False
+    return plan.kind == "rk45" or first or slid
+
+
+def _advect_args(eng, plan, dt, endtime, first, seed, rng_call, rounds, hint=False):
     """The arguments of a round's launch.  AdvectionDiffusionM1 / EM: the iteration count travels with the particle and keys its
     Wiener increments -- the single-GPU run's stream, unchanged by where the rounds cut the call (no round number in the call index).
 
@@ -303,7 +371,7 @@ def _advect_args(eng, plan, dt, endtime, first, seed, rng_call, rounds):
     if plan.kind == "fixed":
         rng_call = (int(rng_call) << 20) + rounds
     return plan.launch_args(eng, dt, endtime, seed=seed, rng_call=rng_call, resume=not first, batch_levels=plan.batch_levels,
-                            next_dt_dtype=plan.next_dt_dtype)  # fmt: skip
+                            hint_all_zero=hint, next_dt_dtype=plan.next_dt_dtype)  # fmt: skip
 
 
 def _advect_round(dfs, args, sign):
@@ -350,8 +418,12 @@ def run_decomposed_p2p(dfs: DecomposedFieldSet, plan, dt: float, endtime: float,
     device = _engine_memory_device(dfs.device)
     sign = 1 if dt > 0 else -1
     stats = dict(rounds=0, migrated=0, particle_steps=0, kernel_ms=0.0, exchange_ms=0.0, transport="peer memory (in-kernel)")
+    slid = False
     for _ in range(max_rounds):
-        rep = _advect_round(dfs, _advect_args(eng, plan, dt, endtime, stats["rounds"] == 0, seed, rng_call, stats["rounds"]), sign)
+        hint = _first_eval_hint(dfs, plan, stats["rounds"] == 0, slid)
+        if dfs.columns and (stats["rounds"] == 0 or slid):
+            _route_columns(dfs, plan, hint, dist, device, stats)
+        rep = _advect_round(dfs, _advect_args(eng, plan, dt, endtime, stats["rounds"] == 0, seed, rng_call, stats["rounds"], hint), sign)
         stats["max_iters_done"] = max(stats.get("max_iters_done", 0), rep["max_iters_done"])
         t0 = time.perf_counter()
         flags = torch.tensor([float(rep["n_migrate"]), float(rep["max_state"] == 99)], dtype=torch.float64,
@@ -367,10 +439,20 @@ def run_decomposed_p2p(dfs: DecomposedFieldSet, plan, dt: float, endtime: float,
         if halo:
             stats["halo_violation"] = True
             raise RuntimeError("halo violation: a stage position left the owned+halo columns; increase halo_cells or reduce dt")
+        slid = moved == 0
         if moved == 0 and not (dfs.fs.time_window is not None and _slide_in_lockstep(dfs, rep, sign, dist, device)):
             break
     _finish_call(dfs, plan, dt, endtime, dist, device, stats)
     return stats
+
+
+def _route_columns(dfs, plan, hint, dist, device, stats):
+    """Column slabs: the set goes to the owners of its cells, with the hint rule of the coming launch, before a launch that skips
+    the hint at the first evaluation (the call's first and, time-windowed, the first after a slide).  A lane the kernel delivered
+    before that evaluation would arrive where the next launch no longer skips the hint, as the single-GPU launch does."""
+    counts = dfs.engine.migrate_classify_columns(hint)
+    _exchange(dfs.engine, counts, dist, device, resume=_carries_resume(plan))
+    stats["migrated"] += int(counts.sum())
 
 
 def _finish_call(dfs, plan, dt, endtime, dist, device, stats):
@@ -400,13 +482,18 @@ def run_decomposed_resident(dfs: DecomposedFieldSet, plan, dt: float, endtime: f
     rep = None
     for _ in range(max_rounds):
         t0 = time.perf_counter()
-        counts = eng.migrate_count()
+        # (column slabs: by the column of the cell each particle's next search finds, with the hint rule of the next launch)
+        counts = eng.migrate_classify_columns(_first_eval_hint(dfs, plan, first, False)) if dfs.columns else eng.migrate_count()
         total, _ = _exchange(eng, counts, dist, device, resume=_carries_resume(plan))
         stats["exchange_ms"] += 1e3 * (time.perf_counter() - t0)
         stats["migrated"] += int(counts.sum())
-        if total == 0 and not first and not (dfs.fs.time_window is not None and _slide_in_lockstep(dfs, rep, sign, dist, device)):
+        slid = total == 0 and not first
+        if slid and not (dfs.fs.time_window is not None and _slide_in_lockstep(dfs, rep, sign, dist, device)):
             break
-        rep = _advect_round(dfs, _advect_args(eng, plan, dt, endtime, first, seed, rng_call, stats["rounds"]), sign)
+        hint = _first_eval_hint(dfs, plan, first, slid)
+        if dfs.columns and slid:  # (the count above used the rule of a launch that does not skip the hint)
+            _route_columns(dfs, plan, hint, dist, device, stats)
+        rep = _advect_round(dfs, _advect_args(eng, plan, dt, endtime, first, seed, rng_call, stats["rounds"], hint), sign)
         first = False
         stats["rounds"] += 1
         stats["particle_steps"] += rep["particle_steps"]
@@ -464,15 +551,17 @@ def download_decomposed(dfs: DecomposedFieldSet, dt: float, ngrids=1, plan=None)
     return {k: v[keep] for k, v in out.items()}
 
 
-def _global_batch_levels(dfs, pdata, dt, endtime, dist, device) -> int:
-    """The reference's batch-level bits of the call's first evaluation (particleset._batch_levels) over the WHOLE set -- every rank's
-    shard -- so that the first-iteration rule of the kernels that count their iterations across ranks is the single-GPU one."""
+def _global_batch_facts(dfs, pdata, dt, endtime, dist, device) -> tuple[bool, int]:
+    """The reference's batch-level decisions of the call's first evaluation (plan.batch_facts) over the WHOLE set -- every rank's
+    shard, one all-reduce: ``hint_all_zero`` (curvilinear grids: every evaluated particle's hinted xi is 0) and the batch-level bits
+    -- so that the first-iteration rules of the kernels are the single-GPU ones."""
     import torch
 
-    _, bits = batch_facts(dfs.fs, pdata, pdata["ei"][:, -1], dt, endtime)
-    v = torch.tensor([float(bits & 1), float(bits & 2)], dtype=torch.float64, device=_collective_device(dist, device))
+    hint_all_zero, bits = batch_facts(dfs.fs, pdata, pdata["ei"][:, -1], dt, endtime)
+    v = torch.tensor([float(bits & 1), float(bits & 2), float(not hint_all_zero)], dtype=torch.float64,
+                     device=_collective_device(dist, device))  # fmt: skip
     dist.all_reduce(v, op=dist.ReduceOp.MAX)
-    return int(v[0].item() > 0) | (2 if v[1].item() > 0 else 0)
+    return v[2].item() == 0, int(v[0].item() > 0) | (2 if v[1].item() > 0 else 0)
 
 
 def execute_decomposed(dfs: DecomposedFieldSet, pdata: dict, kernels, dt: float, endtime: float, dist, max_rounds=100000, seed=0,
@@ -481,8 +570,12 @@ def execute_decomposed(dfs: DecomposedFieldSet, pdata: dict, kernels, dt: float,
     routed to the owners first).  Returns (local particle dict after the call, stats)."""
     plan = decomposed_plan(dfs, kernels, pdata)
     upload_decomposed(dfs, pdata, dt, plan)
-    if _carries_resume(plan) or dfs.fs.interp_method != "linear":  # (fixed-step XLinear_Velocity lists keep the plan's 0)
-        plan.batch_levels = _global_batch_levels(dfs, pdata, dt, endtime, dist, _engine_memory_device(dfs.device))
+    if dfs.columns and allreduce_sum(len(pdata["x"]), dist, _collective_device(dist, _engine_memory_device(dfs.device))) == 1:
+        # (a set of one particle is its own batch for the reference's `if np.any(xi)` at every evaluation: a rule of the whole set
+        #  that the engine of a shard does not apply)
+        raise NotImplementedError("a particle set of ONE particle on a curvilinear grid runs on one GPU, not on column slabs")
+    if _carries_resume(plan) or dfs.fs.interp_method != "linear" or dfs.columns:  # (rectilinear fixed-step XLinear_Velocity: 0)
+        plan.hint_all_zero, plan.batch_levels = _global_batch_facts(dfs, pdata, dt, endtime, dist, _engine_memory_device(dfs.device))
     if dfs.fs.time_window is not None:
         # first window: where the earliest (latest, backward in time) particle of ANY rank starts -- the same on every rank
         import torch

@@ -345,10 +345,30 @@ class Engine:
         check(self._lib.pb_decomp_set(self._h, int(nranks), int(rank), ptr(b), int(xi_offset), int(left_is_global),
                                       int(right_is_global)))  # fmt: skip
 
+    def decomp_set_columns(self, nranks, rank, col_edges, xi_offset, left_is_global, right_is_global):
+        """Column slabs of a curvilinear grid (pb_decomp_set_columns): ``col_edges`` are the nranks + 1 cell-column edges."""
+        c = np.ascontiguousarray(col_edges, dtype=np.int64)
+        assert c.size == nranks + 1
+        self._nranks = int(nranks)
+        check(self._lib.pb_decomp_set_columns(self._h, int(nranks), int(rank), ptr(c), int(xi_offset), int(left_is_global),
+                                              int(right_is_global)))  # fmt: skip
+
     def migrate_count(self) -> np.ndarray:
         counts = np.zeros(self._nranks, dtype=np.int64)
         check(self._lib.pb_migrate_count(self._h, ptr(counts)))
         return counts
+
+    def migrate_classify_columns(self, no_hint: bool) -> np.ndarray:
+        """``migrate_count`` of column slabs: leavers per rank by the column of the cell each particle's next search finds."""
+        counts = np.zeros(self._nranks, dtype=np.int64)
+        check(self._lib.pb_migrate_classify_columns(self._h, int(bool(no_hint)), ptr(counts)))
+        return counts
+
+    def memory_bytes(self) -> tuple[int, int]:
+        """(grid bytes, field bytes) the engine holds on its device."""
+        g, f = np.zeros(1, dtype=np.int64), np.zeros(1, dtype=np.int64)
+        check(self._lib.pb_memory_bytes(self._h, ptr(g), ptr(f)))
+        return int(g[0]), int(f[0])
 
     def migrate_pack(self, sendbuf_ptr: int, capacity_records: int):
         check(self._lib.pb_migrate_pack(self._h, C.c_void_p(sendbuf_ptr), int(capacity_records)))

@@ -199,6 +199,7 @@ class KernelPlan:
         self.kh, self.kh_spherical, self.kh_deg2m = (0.0, 0.0), False, 1.0
         self.next_dt_dtype = None  # (AdvectionRK45: the dtype of the next_dt Variable)
         self.batch_levels = 0  # the call's batch-level bits where all launches of a call share them (mode D, distributed.py)
+        self.hint_all_zero = False  # mode D on column slabs: the whole set's hint_all_zero of the call's first evaluation
         if "AdvectionRK45" in tokens:
             self._setup_rk45(names, fieldset, pclass)
             # [AdvectionRK45] or [AdvectionRK45, DeleteParticle]: the whole loop in one launch.  Mixed with user kernels (the

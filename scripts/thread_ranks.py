@@ -45,6 +45,21 @@ class ThreadGroup:
                 group.barrier.wait()  # everybody has read the slots before the next collective overwrites them
                 t.copy_(res)
 
+            @staticmethod
+            def all_gather_into_tensor(out, t):
+                group.slots[rank] = t.clone()
+                group.barrier.wait()
+                res = torch.cat(group.slots)
+                group.barrier.wait()
+                out.copy_(res)
+
+            @staticmethod
+            def all_gather_object(out, obj):
+                group.slots[rank] = obj
+                group.barrier.wait()
+                out[:] = list(group.slots)
+                group.barrier.wait()
+
         return Member
 
 
