@@ -129,7 +129,7 @@ def build(force: bool = False) -> str:
         if p.returncode != 0:
             raise RuntimeError(f"hostsim compile failed:\n{' '.join(cmd)}\n{o}\n{e[:6000]}")
         objs.append(obj)
-    res = subprocess.run([cxx, "-shared", "-o", OUT, *objs], capture_output=True, text=True)
+    res = subprocess.run([cxx, "-shared", "-o", OUT, *objs, "-ldl"], capture_output=True, text=True)
     if res.returncode != 0:
         raise RuntimeError(f"hostsim link failed:\n{res.stdout}\n{res.stderr[:4000]}")
     return OUT

@@ -15,6 +15,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <dlfcn.h>
 
 #define PB_HOSTSIM 1
 #define __global__
@@ -172,9 +173,23 @@ inline cudaError_t cudaEventElapsedTime(float* ms, cudaEvent_t a, cudaEvent_t b)
 template <class F>
 inline cudaError_t cudaFuncSetAttribute(F, int, int) { return cudaSuccess; }
 
+// Opt-in launch trace: when PB_HOSTSIM_TRACE names a file, every launch appends the (mangled) symbol of its kernel to it, one per
+// line, so that a test can tell which template instantiations a run launched.  Without the variable it does nothing.
+inline void hs_trace(const void* f) {
+    const char* path = std::getenv("PB_HOSTSIM_TRACE");
+    if (!path || !path[0]) return;
+    Dl_info info;
+    if (!dladdr(f, &info) || !info.dli_sname) return;
+    if (FILE* out = std::fopen(path, "a")) {
+        std::fprintf(out, "%s\n", info.dli_sname);
+        std::fclose(out);
+    }
+}
+
 // ---- kernel launches: build.py rewrites `k<<<grid, block, smem, stream>>>(args)` into HS_LAUNCH((k), grid, block, smem, stream, args)
 template <class F, class... Args>
 inline void hs_launch(F f, unsigned long long grid, unsigned long long block, Args... args) {
+    hs_trace((const void*)f);
     const unsigned long long n = grid * block;  // kernels index with blockIdx.x * blockDim.x + threadIdx.x and guard i < n themselves
     blockDim.x = 1; gridDim.x = (unsigned)n; threadIdx.x = 0;
     for (unsigned long long i = 0; i < n; ++i) {

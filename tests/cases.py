@@ -245,9 +245,10 @@ def build(spec):
         depth = (np.linspace(0, 1, nz) ** 1.4 * 200.0).astype(cd) if nz > 1 else None
         shape = (nt, nz, ny, nx)
         umax = spec["umax"]
-        U = (umax * rng.uniform(-1, 1, shape)).astype(np.float32)
-        V = (umax * rng.uniform(-1, 1, shape)).astype(np.float32)
-        W = (1e-2 * rng.uniform(-1, 1, shape)).astype(np.float32) if three_d else None
+        dd = np.dtype(spec.get("ddtype", "f4"))  # float32 velocity data unless the spec asks for another dtype
+        U = (umax * rng.uniform(-1, 1, shape)).astype(dd)
+        V = (umax * rng.uniform(-1, 1, shape)).astype(dd)
+        W = (1e-2 * rng.uniform(-1, 1, shape)).astype(dd) if three_d else None
         x, y = points_in_mesh(rng, lon, lat, n)
         if spec.get("wrap_lon"):  # nodes and releases wrapped to [-180, 180) after the releases were blended
             lon = (((lon.astype(np.float64) + 180.0) % 360.0) - 180.0).astype(cd)
